@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — queries/sec @ recall@10, DBpedia-1M-shaped d=768 top-10 (BASELINE.json), on 1/2/4/8 B200.
+"""bench.py — queries/sec @ recall@10, DBpedia-1M-shaped d=768 top-10 (BASELINE.json), on 1/2/4/8 H100.
 
 A "step" is one pass of the hot path over one batch of Q independent single-query HNSW traversals
 (config C2: 1M x 768 f32, cosine, m=16/m0=32/ef_construction=200, ef=100, k=10; no cross-query sharing).
@@ -8,7 +8,7 @@ A "step" is one pass of the hot path over one batch of Q independent single-quer
   e2e     : the same metric through the reference-facing C-ABI call hx_search with HOST (pinned) buffers:
             H2D of the queries and D2H of ids/scores/counts are inside the timed region.
   roofline: k_hnsw_search, algorithmic bytes E*(5+8*32) + Dc*(4+4d) per launch (SURVEY §8d) / CUDA-event kernel time,
-            against the measured HBM peak in MEASURED_PEAKS.json.
+            against the measured HBM peak in MEASURED_PEAKS.json (else the H100 SXM data sheet's 3.35 TB/s).
   cpu_baseline / --impl reference: the CPU oracle (restatement of the reference's algorithm without its KV layer)
             traversing the IDENTICAL graph on all host cores, one query per thread.
   N > 1   : one process per GPU (torchrun).  `value` is the "replica" mode: the QUERIES are partitioned across full
@@ -49,7 +49,7 @@ EF = 100
 #      sentence embeddings; HNSW (m=16, ef=100) reaches recall@10 ~0.97 on it, as it does on DBpedia-OpenAI-1M.
 #  "survey": SURVEY §8(d)'s literal example — 1024 isolated isotropic clusters in full 768-d (sigma 0.3).  Its landscape is
 #      flat between clusters, so ANY greedy HNSW descent (reference algorithm included) lands in a wrong cluster for ~7 %
-#      of the queries at 1M (profiles/r01_recall_diag_survey_mixture.json): recall@10 0.89 at ef=100, 0.91 at ef=200.
+#      of the queries at 1M, so recall@10 stays near 0.9 even at ef=200.
 RECIPES = {"embedding": dict(kind=32, sigma=1.0), "survey": dict(kind=0, sigma=0.3)}
 KIND = 32
 SIGMA = 1.0
@@ -78,6 +78,8 @@ def parse():
     ap.add_argument("--dense-batch", type=int, default=1024)
     ap.add_argument("--callers-seconds", type=float, default=1.0)
     ap.add_argument("--recipe", default="embedding", choices=sorted(RECIPES))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's answer of the headline HNSW path (ids, scores, counts) as DIR/<name>.npy")
     a = ap.parse_args()
     global KIND, SIGMA
     KIND, SIGMA = RECIPES[a.recipe]["kind"], RECIPES[a.recipe]["sigma"]
@@ -85,7 +87,7 @@ def parse():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
     def __init__(self, device_index: int):
         self.idx = device_index
@@ -157,7 +159,7 @@ def measured_peaks():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def ncu_traffic(kernel: str, shape: dict):
@@ -249,13 +251,33 @@ def c2_config(args, world):
         "queries_per_step_per_gpu": Q,
         "parallelism": "single GPU" if world == 1 else f"{world} full replicas, queries partitioned, no data-path collective",
         "value_mode": "single GPU" if world == 1 else "replicas (the id-range-sharded path is the `sharded` object)",
-        "l2": f"corpus {n * dim * 4 / 1e9:.2f} GB >> 126 MB L2; distinct queries every step and rank",
+        "l2": f"corpus {n * dim * 4 / 1e9:.2f} GB >> 50 MB L2; distinct queries every step and rank",
         "graph": "built on the device (hx_index_build), identical adjacency mirrored into the CPU oracle",
         "data_recipe": (f"{args.recipe}: unit-normalised {N_CENTROIDS}-component Gaussian mixture, sigma={SIGMA}, "
                         + (f"rank-{KIND} latent space -> fixed random projection to {dim}-d + 2% noise"
                            if KIND else f"isolated isotropic clusters in {dim}-d") + ", seed=0x0DB9ED1A"),
     }
     return cfg
+
+
+def dump_outputs(out_dir, o_ids, o_sc, o_cnt, cap_bytes=64 << 20):
+    """What a caller of hx_search_device receives for the step: ids (float64: exact below 2**53), scores (float32) and
+    result counts per query, as .npy files (32768 queries x k=10: 4.2 MB).  Above `cap_bytes` a fixed, seeded sample of
+    the queries is written, with their indices in query_index.npy."""
+    ids = o_ids.cpu().numpy().view(np.uint64).astype(np.float64)
+    sc = o_sc.cpu().numpy().astype(np.float32)
+    cnt = o_cnt.cpu().numpy().astype(np.float64)
+    q = len(cnt)
+    per_query = ids.shape[1] * 12 + 16
+    rows = np.arange(q)
+    if q * per_query > cap_bytes:
+        rows = np.sort(np.random.default_rng(SEED).choice(q, cap_bytes // per_query, replace=False))
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "ids.npy", ids[rows])
+    np.save(d / "scores.npy", sc[rows])
+    np.save(d / "counts.npy", cnt[rows])
+    np.save(d / "query_index.npy", rows.astype(np.float64))
 
 
 def recall_at_k(found, truth):
@@ -447,9 +469,9 @@ def measure_prefilter(hx, torch, ix, args, dev, stream, n, dim, ora=None, label_
             cset = hx.RestrictedVectorCandidates(cids)
             fst = hx.FilteredStats()
             try:
-                # one CTA per query: 296 queries per call fill the 148 SMs twice over (the 64-query step above would leave
+                # one CTA per query: 264 queries per call fill the 132 SMs twice over (the 64-query step above would leave
                 # more than half of them idle); both plans are timed through the same host entry points on the same queries
-                AB = 296
+                AB = 264
                 aq = ix.generate_queries(SEED, AB, first_query=22_000_000, n_centroids=N_CENTROIDS, sigma=SIGMA, kind=KIND)
                 x_ids, _, x_cnt = ix.search_restricted_batch(aq, params, cset)
                 t0 = time.perf_counter()
@@ -501,7 +523,7 @@ def measure_prefilter(hx, torch, ix, args, dev, stream, n, dim, ora=None, label_
         "recall_at_10": 1.0, "dtype": "f32",
         "config": {"workload": f"C3: {n}x{dim} f32 {args.metric}, {B} queries per step, query b restricted to "
                                f"{{id : id mod {sel} == b}} ({per_q} candidates each): every row read once per step",
-                   "l2": f"{n * dim * 4 / 1e9:.2f} GB streamed per step >> 126 MB L2"},
+                   "l2": f"{n * dim * 4 / 1e9:.2f} GB streamed per step >> 50 MB L2"},
         "e2e": {"value": round(e2e_value, 1), "unit": "queries/s", "h2d_bytes_per_step": B * dim * 4 + total * 8 + (B + 1) * 8,
                 "d2h_bytes_per_step": B * (k * 12 + 4) + B * 4 + 4, "api": "hx_search_restricted_multi (C ABI, pinned host)",
                 "identical_to_device_path": same},
@@ -558,7 +580,7 @@ def measure_callers(hx, ix, queries, k, ef, seconds):
 
 def measure_dense(hx, torch, args, world, rank, local_rank, dev, stream, uid):
     """C4 shape: exhaustive top-10 of a 1024-query batch against 1.25M x 768 bf16 rows PER GPU through the tensor cores
-    (k_dense_scores: tcgen05 + TMEM + TMA), nominees re-ranked by the exact fp32 scan; with N > 1 the corpus is the
+    (k_dense_scores: wgmma + TMA), nominees re-ranked by the exact fp32 scan; with N > 1 the corpus is the
     id-range union of the ranks' shards (8 GPUs = C4's 10M rows) and every step ends with ONE ncclAllGather + merge
     (hx_search_sharded*, issued by the library)."""
     from helix_db_b200 import sharding as sh
@@ -575,7 +597,7 @@ def measure_dense(hx, torch, args, world, rank, local_rank, dev, stream, uid):
         uid = sh.exchange_unique_id(rank, device=dev)
     g = sh.ShardGroup(ix, world, rank, uid)
     peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text()) if (ROOT / "MEASURED_PEAKS.json").exists() else {}
-    tf_peak = float(peaks.get("bf16_tflops", 1590.0))
+    tf_peak = float(peaks.get("bf16_tflops", 989.0))
     steps = args.steps
     qsets = [ix.generate_queries(SEED, B, first_query=30_000_000 + s * B, n_centroids=N_CENTROIDS, sigma=SIGMA, kind=KIND)
              for s in range(steps + args.warmup)]          # every rank answers the SAME queries
@@ -636,7 +658,7 @@ def measure_dense(hx, torch, args, world, rank, local_rank, dev, stream, uid):
     out = {"metric": "queries/sec, exhaustive top-10 through the tensor cores (config C4 shape)",
            "value": round(steps * B / (ms_total / 1e3), 1), "unit": "queries/s", "n_gpus": world, "steps": steps,
            "ms_per_step": round(ms_total / steps, 3), "scaling": "weak (rows per GPU fixed; 8 GPUs = C4's 10M rows)",
-           "dtype": "bf16 (fp32 accumulate in TMEM) + f32 exact re-rank", "recall_at_10_vs_exact_scan": round(rec, 4),
+           "dtype": "bf16 (fp32 accumulate) + f32 exact re-rank", "recall_at_10_vs_exact_scan": round(rec, 4),
            "config": {"workload": f"C4 shard shape: {B} queries x {rows} rows per GPU x d={dim} (total {rows * world} rows on "
                                   f"{world} GPU(s)), k={k}", "setup": {"generate_s": round(gen_s, 2)}},
            "e2e": {"value": round(steps * B / wall, 1), "unit": "queries/s", "ms_per_step": round(wall / steps * 1e3, 3),
@@ -651,7 +673,7 @@ def measure_dense(hx, torch, args, world, rank, local_rank, dev, stream, uid):
                         "peak": tf_peak, "unit": "TFLOP/s", "frac": round(flop / (kernel_ms * 1e-3) / 1e12 / tf_peak, 4) if kernel_ms else None,
                         "traffic": ncu_traffic("k_dense_scores", {"queries": B, "rows": rows, "dim": dim}),
                         "flop_per_launch_per_gpu": flop, "kernel_ms_per_launch": round(kernel_ms, 4),
-                        "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst); per GPU"},
+                        "peak_source": "MEASURED_PEAKS.json bf16_tflops, else the H100 SXM data sheet's dense bf16 989; per GPU"},
            "gpu_launches": steps * 8}
     if world == 1 and rank == 0 and not args.no_cpu:
         # the oracle's exact scan (search_exact = restricted_exact_scan over every id) on a bounded sample: parity + CPU rate
@@ -839,6 +861,8 @@ def run_ours(args):
     barrier()
     clocks = sampler.stop() if rank == 0 else None
     ms_total = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:   # the last timed step's answer, before anything below reuses the output buffers
+        dump_outputs(args.dump_outputs, o_ids, o_sc, o_cnt)
     kernel_ms_total, kernel_launches = ix.last_kernel_ms()
     dev_flags, dev_flag_status = ix.device_flags(stream)   # error flags ORed over the timed launches (ADVICE r1): must be 0
     if dev_flags != 0:
@@ -1096,7 +1120,7 @@ def run_ours(args):
     line = None
     if rank == 0:
         line = {
-            "metric": "queries/sec @ recall@10, DBpedia-1M d=768 top-10, 1/2/4/8 B200 vs CPU ref",
+            "metric": "queries/sec @ recall@10, DBpedia-1M d=768 top-10, 1/2/4/8 H100 vs CPU ref",
             "value": round(value, 1), "unit": "queries/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": round(ms_total / args.steps, 4), "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -1282,7 +1306,7 @@ def run_reference(args):
     rec = recall_at_k(last[0][:min(rq, per_step)], truth[:min(rq, per_step)])
     line = {
         "impl": "reference",
-        "metric": "queries/sec @ recall@10, DBpedia-1M d=768 top-10, 1/2/4/8 B200 vs CPU ref",
+        "metric": "queries/sec @ recall@10, DBpedia-1M d=768 top-10, 1/2/4/8 H100 vs CPU ref",
         "value": round(value, 1), "unit": "queries/s", "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": round(total / args.steps * 1e3, 3), "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f32", "data": "synthetic", "recall_at_10": round(rec, 4),

@@ -1,4 +1,4 @@
-"""helix-db_b200 — host-side mirror of HelixDB's vector-index read API over the B200 C ABI.
+"""helix-db_b200 — host-side mirror of HelixDB's vector-index read API over the C ABI of libhelix_b200 (CUDA, sm_90a).
 
 The reference's production vector queries funnel through
 ``ValidatedVectorReadIndex::<D>::{search, search_restricted}``

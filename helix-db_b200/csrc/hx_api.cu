@@ -35,7 +35,7 @@ void hx_set_error_index(uint32_t idx) { g_err_index = idx; }
 
 extern "C" const char* hx_last_error(void) { return g_err; }
 extern "C" uint32_t hx_last_error_index(void) { return g_err_index; }
-extern "C" const char* hx_version(void) { return "helix_b200 0.1 (sm_100a)"; }
+extern "C" const char* hx_version(void) { return "helix_b200 0.1 (sm_90a)"; }
 
 // ------------------------------------------------------------------------------------------------
 // helpers
@@ -1388,7 +1388,7 @@ static hx_status launch_hnsw(hx_index* ix, HxScratch* s, const float* d_queries,
     rg.prefetch_below = knob(t.prefetch_below, ef / 2 + 1);
     if ((rc = setup_tie_pool(s, &rg, stream))) return rc;
     rg.batch_admit = knob(t.lat_admit_seq, 0) ? 0u : 1u;
-    rg.l2_spec = knob(t.lat_spec, 0);   // measured: the speculative row prefetch costs more than it hides (profiles/r01_latency_*)
+    rg.l2_spec = knob(t.lat_spec, 0);   // off: the speculative row prefetch costs more than it hides (DESIGN §5)
     if (knob(t.phase_prof, 0)) {        // diagnostics: cycle sums per phase of the latency build
       if ((rc = s->d_prof.reserve(8))) return rc;
       if (!s->prof_init) { HX_CUDA(cudaMemsetAsync(s->d_prof.p, 0, 8 * sizeof(unsigned long long), stream)); s->prof_init = true; }
@@ -2442,7 +2442,7 @@ static hx_status launch_policy(hx_index* ix, HxScratch* s, const float* d_querie
   const uint32_t fr_cap = round_up(std::max(ix->stride0, ix->stride_u), 32);
   const size_t rowbytes = (size_t)ix->ld * 4;
   // the query stays in shared memory: holding it in registers (QCH = 24) spills at the 128-register cap of a 512-thread CTA
-  // and measured 2x slower (profiles/r01_policy_sweep.json)
+  // and was slower
   const uint32_t pol_qch = 0;
   const size_t fixed0 = (pol_qch ? 0 : rowbytes) + (size_t)ef * 8 + (size_t)k * 8 + HX_TIE_CAP * 8 + (size_t)fr_cap * 13 +
                         28 * 4 + 16;

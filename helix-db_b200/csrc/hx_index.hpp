@@ -141,7 +141,7 @@ struct hx_index {
   hx_index_config cfg{};
   hx_tuning tune{};   // launch-shape knobs: environment at hx_index_create, hx_index_set_tuning afterwards
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   uint32_t lim0 = 32;   // MutationDegreeLimits.layer0 = max(m0, 2m)  (mutation.rs:179-199)
   // vectors
   size_t n = 0;

@@ -2,23 +2,20 @@
 //
 // The only place on this hot path where the work is a dense contraction: S[b][i] = <q_b, x_i> for B = 1024..4096
 // queries against the whole shard is a (B x d) x (d x N) GEMM with arithmetic intensity ~B flop/byte, far beyond the
-// HBM ridge.  It runs on the 5th-generation tensor cores:
-//   * operands in bf16 (a bf16 copy of the corpus is kept when hx_index_config.storage == 1), fp32 accumulation in TMEM;
-//   * CTA PAIRS (thread-block clusters of 2 = the two SMs of a TPC): one tcgen05.mma.cta_group::2 covers 256 queries x 256
-//     corpus rows x 16 (K) — each CTA holds its own 128 queries (A, and the 128 TMEM lanes of their accumulators) and
-//     stages only HALF of the corpus tile (B); the tensor cores of both SMs read both halves.  With cta_group::1 every SM
-//     staged the whole 48 KB k-block itself: 94 B/clk of TMA writes + 94 B/clk of operand reads against 128 B/clk of shared
-//     memory bandwidth — ncu: tensor pipe 65 % of active (profiles/r02_ncu_dense_v2_details.txt).  Pairing cuts both to
-//     64 + 64 KB per 2 SMs;
-//   * 5-stage TMA ring of (16 KB A | 16 KB half-B) per CTA (cp.async.bulk.tensor.cta_group::2, 128-byte swizzle, completion
-//     counted on the LEADER CTA's mbarrier), MMAs issued by one elected thread of the leader, ring slots and accumulator
-//     stages released in both CTAs by multicast tcgen05.commit; accumulators double-buffered in TMEM (2 x 256 columns);
-//   * fused epilogue: 16 warps per CTA (one per TMEM lane quarter x column quarter) read the accumulator with tcgen05.ld,
-//     turn it into the metric's score order with the stored row norms, and keep the HX_DENSE_T best rows per (query, run of
-//     tiles, column quarter) by register insertion, emitting score_bits<<32|slot keys — the B x N score matrix is never
-//     written.  The epilogue is what bounds the kernel at K = 768: a warp's column work is one dependent instruction
-//     stream, and with 8 warps it took longer per tile than the tile's MMAs (1.60 ms, 0.78 of the burst peak); with 16
-//     warps 1.45 ms, 0.86 (profiles/r02_dense_limiter_experiments.json).
+// HBM ridge.  It runs on the Hopper tensor cores (sm_90a):
+//   * operands in bf16 (a bf16 copy of the corpus is kept when hx_index_config.storage == 1), fp32 accumulation in the
+//     registers of the issuing warpgroup;
+//   * one persistent CTA per SM.  A producer warp streams (128 queries | 128 corpus rows) x 64-element k-blocks with TMA
+//     (128-byte swizzle) into a 4-stage shared-memory ring whose slots are handed over by mbarriers (full: bytes landed,
+//     empty: the MMAs that read the slot have completed).  Two consumer warpgroups each issue wgmma.m64n128k16 for 64 of
+//     the 128 queries with both operands read straight from shared memory, keeping one wgmma group in flight while the
+//     next slot is waited for;
+//   * fused epilogue: the accumulators of each 128 x 128 half tile are written to shared memory (row stride 129 floats, so
+//     the column-order reads below are free of bank conflicts); each of the 256 consumer threads — one query row x one
+//     64-column quarter — turns them into the metric's score order with the stored row norms and keeps the HXD_T best rows
+//     per (query, run of tiles, column quarter) by register insertion, emitting score_bits<<32|slot keys — the B x N
+//     score matrix is never written.  Per half tile the epilogue is 64 columns per thread against the 4 x ldb/64 wgmma
+//     steps of the contraction, so it runs between the MMAs of consecutive half tiles instead of beside them.
 // The approximate (bf16) keys only NOMINATE candidates: k_select keeps the k' best keys per query and the exact fp32
 // scan kernel (bit-exact reference arithmetic) re-ranks them, so returned scores are exact and ordering follows the
 // reference's (score, id) rule; recall vs the exhaustive exact scan is measured, not assumed.
@@ -37,11 +34,12 @@
 #include "k_scan.cuh"
 #include "k_util.cuh"
 
-#define HXD_BM 128          // queries per CTA tile (UMMA M = 256 over the CTA pair)
-#define HXD_BN 256          // corpus rows per tile (UMMA N); each CTA of the pair stages HXD_BN / 2 of them
+#define HXD_BM 128          // queries per CTA tile: two consumer warpgroups x 64 (wgmma M)
+#define HXD_BN 256          // corpus rows per placement tile (the unit of the row interleave and of the column quarters)
+#define HXD_BH 128          // corpus rows per MMA tile (wgmma N): a placement tile is contracted in two halves
 #define HXD_BK 64           // bf16 elements per k-block = 128 bytes = one swizzle atom
-#define HXD_STAGES 5
-#define HXD_PARTS 4         // column quarters of a tile: one epilogue warp per (TMEM lane quarter, column quarter)
+#define HXD_STAGES 4
+#define HXD_PARTS 4         // 64-column quarters of a placement tile: one bucket of the fused top-T per (query, run, quarter)
 #ifndef HXD_T
 #define HXD_T 8             // best rows kept per (query, run of n-tiles, column quarter): 32 per (query, run)
 #endif
@@ -50,10 +48,8 @@
 // ids (near-duplicate rows inserted back to back: chunks of one document) could have more than HXD_T of them in one bucket and
 // lose the rest.  HXD_INTERLEAVE = 1 stores row j of a tile at position (j % 4) * 64 + j / 4: consecutive ids land in different
 // quarters (a run of 32 consecutive ids puts at most 8 into any bucket), at no cost to the kernel (same loads, same MMAs; only
-// the slot a column stands for changes).
-// Measured (profiles/r02_dense_row_placement_ab.json): on a fixture whose 11 nearest rows are consecutive ids the id-order
-// placement returns 8 of the 10 true neighbours (recall 0.8), the interleaved one all of them; kernel time 1.489 -> 1.458 ms at
-// the C4 shard shape (no cost).  Default on.
+// the slot a column stands for changes).  tests/test_gpu_zz_reference_contracts.py::test_dense_path_keeps_id_clustered_neighbours
+// is the fixture on which id order loses neighbours.  Default on.
 #ifndef HXD_INTERLEAVE
 #define HXD_INTERLEAVE 1
 #endif
@@ -72,115 +68,54 @@ __host__ __device__ __forceinline__ uint32_t hxd_row_at_pos(uint32_t c) {
   return c;
 #endif
 }
-#define HXD_THREADS 640     // warp 0: TMA, warp 1: MMA, warp 2: TMEM alloc, warp 3: idle, warps 4-19: epilogue
-#define HXD_EPI_THREADS 512
-#define HXD_STAGE_CAP 12    // per-thread staging entries (shared memory) between the column test and the top-T insertion
+#define HXD_CONSUMERS 256   // warps 0-7: two consumer warpgroups (MMA + epilogue); warp 8: TMA producer
+#define HXD_THREADS (HXD_CONSUMERS + 32)
 #define HXD_A_BYTES (HXD_BM * HXD_BK * 2)
-#define HXD_B_BYTES ((HXD_BN / 2) * HXD_BK * 2)   // this CTA's half of the corpus tile
+#define HXD_B_BYTES (HXD_BH * HXD_BK * 2)
 #define HXD_STAGE_BYTES (HXD_A_BYTES + HXD_B_BYTES)
+#define HXD_ACC_LD (HXD_BH + 1)   // floats per row of the accumulator tile in shared memory
 
 // ---- PTX wrappers ------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t hxd_cta_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t hxd_mapa(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void hxd_cluster_sync() {   // all threads of both CTAs
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// tile -> this CTA's shared memory; the bytes are counted on the mbarrier at cluster address `bar_cluster` (the leader's)
-__device__ __forceinline__ void hxd_tma_load_2d(void* smem_dst, const CUtensorMap* map, uint32_t bar_cluster, int c0, int c1) {
+// tile -> shared memory; the bytes are counted on `bar`
+__device__ __forceinline__ void hxd_tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
           hx_smem_u32(smem_dst)),
-      "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1)
+      "l"(map), "r"(hx_smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
 __device__ __forceinline__ void hxd_prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void hxd_mbar_arrive_cluster(uint32_t bar_cluster) {   // arrive on a barrier of any CTA of the cluster
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
+__device__ __forceinline__ void hxd_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void hxd_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void hxd_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// ties the accumulator registers to the surrounding asm so that no read of them moves across a wgmma wait
+__device__ __forceinline__ void hxd_fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void hxd_tmem_alloc(uint32_t* smem_out, uint32_t cols) {   // the same warp id in both CTAs of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(hx_smem_u32(smem_out)), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void hxd_tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void hxd_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void hxd_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// D[tmem of both CTAs] (+)= A[smem of both CTAs] * B[smem halves of both CTAs]^T, M=256, N=256, K=16 (bf16), fp32 accumulate.
-// Issued by one thread of the leader CTA; the descriptors are shared-memory offsets valid in both CTAs.
-__device__ __forceinline__ void hxd_umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, bf16 operands from shared memory (both K-major), fp32 accumulate in registers.
+// Thread layout of D (warp w of the warpgroup, lane l): d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e].
+__device__ __forceinline__ void hxd_wgmma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued MMAs of this thread arrive on the barrier at the same offset in BOTH CTAs when they have completed
-__device__ __forceinline__ void hxd_umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   hx_smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i = TMEM lane base+i)
-__device__ __forceinline__ void hxd_tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// the same load without the wait: the caller overlaps it with work on the previous chunk, then hxd_tmem_wait_ld()
-__device__ __forceinline__ void hxd_tmem_ld32_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void hxd_tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 8 consecutive fp32 columns
-__device__ __forceinline__ void hxd_tmem_ld8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
 // K-major operand tile stored by TMA with the 128-byte swizzle: rows of 128 bytes, 8-row groups 1024 bytes apart.
-// SmemDescriptor (cute/arch/mma_sm100_desc.hpp): start>>4 [0,14) | LBO>>4 [16,30) = 1 | SBO>>4 [32,46) = 64 |
-// version [46,48) = 1 (Blackwell) | layout_type [61,64) = 2 (SWIZZLE_128B).
+// wgmma matrix descriptor: start>>4 [0,14) | LBO>>4 [16,30) = 1 (unused for swizzled K-major) | SBO>>4 [32,46) = 64 |
+// base offset [49,52) = 0 (tiles are 1024-byte aligned) | layout [62,64) = 1 (SWIZZLE_128B).
 __device__ __forceinline__ uint64_t hxd_make_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);
   d |= (uint64_t)1u << 16;
   d |= (uint64_t)64u << 32;
-  d |= (uint64_t)1u << 46;
-  d |= (uint64_t)2u << 61;
+  d |= (uint64_t)1u << 62;
   return d;
 }
 
@@ -188,235 +123,174 @@ struct HxDenseArgs {
   uint32_t n_rows;            // corpus rows (unpadded)
   uint32_t n_queries;         // B (unpadded)
   uint32_t k_blocks;          // ldb / 64
-  uint32_t m_pairs, n_tiles;  // m_pairs = pairs of 128-query tiles (one pair = one CTA pair)
-  uint32_t n_split;           // work unit u of a CTA pair: query pair u % m_pairs, n-tiles [r*n_tiles/n_split, (r+1)*n_tiles/n_split), r = u / m_pairs
+  uint32_t m_tiles, n_tiles;  // 128-query tiles, 256-row corpus tiles
+  uint32_t n_split;           // work unit u: query tile u % m_tiles, n-tiles [r*n_tiles/n_split, (r+1)*n_tiles/n_split), r = u / m_tiles
   const float* row_aux;       // cosine: 1/|x_i|   ; euclidean: |x_i|^2            (from the bf16-rounded rows)
   const float* q_aux;         // cosine: 1/|q_b|   ; euclidean: |q_b|^2
   uint64_t* keys;             // [B][n_split][HXD_PARTS][HXD_T]
   int32_t metric;
 };
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(HXD_THREADS, 1)
+// insert (t, slot) into a descending best-T list (ties keep the earlier column)
+__device__ __forceinline__ void hxd_insert(float (&bt)[HXD_T], uint32_t (&bs)[HXD_T], float t, uint32_t slot) {
+  bt[HXD_T - 1] = t;
+  bs[HXD_T - 1] = slot;
+#pragma unroll
+  for (int j = HXD_T - 1; j > 0; --j)
+    if (bt[j] > bt[j - 1]) {
+      const float tf = bt[j]; bt[j] = bt[j - 1]; bt[j - 1] = tf;
+      const uint32_t tsl = bs[j]; bs[j] = bs[j - 1]; bs[j - 1] = tsl;
+    }
+}
+
+__global__ void __launch_bounds__(HXD_THREADS, 1)
 k_dense_scores(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x, HxDenseArgs a) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  // HXD_STAGES x (A 16 KB | half-B 16 KB); the 128-byte swizzle needs 1024-byte aligned tiles: align inside the window
-  // (the window starts at the same offset in both CTAs of the pair, so every object below has the same offset in both)
+  // HXD_STAGES x (A 16 KB | B 16 KB); the 128-byte swizzle needs 1024-byte aligned tiles: align inside the window
   unsigned char* smem = smem_raw + ((1024u - (hx_smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* tiles = smem;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + HXD_STAGES * HXD_STAGE_BYTES);   // leader's copy is the live one
-  uint64_t* empty = full + HXD_STAGES;      // per CTA: ring slot free (multicast commit of the MMAs that read it)
-  uint64_t* tfull = empty + HXD_STAGES;     // [2] per CTA: accumulator stage ready for the epilogue (multicast commit)
-  uint64_t* tempty = tfull + 2;             // [2] leader's copy: accumulator stage drained by the epilogues of BOTH CTAs
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* aux = reinterpret_cast<float*>(tmem_slot + 4);   // [2][HXD_BN] row aux of the tile being drained
-  float* stg_t = aux + 2 * HXD_BN;                          // [HXD_STAGE_CAP][256] staged t values   (entry-major: conflict-free)
-  uint32_t* stg_s = reinterpret_cast<uint32_t*>(stg_t + HXD_STAGE_CAP * HXD_EPI_THREADS);   // [HXD_STAGE_CAP][256] staged slots
+  float* accs = reinterpret_cast<float*>(smem + HXD_STAGES * HXD_STAGE_BYTES);   // [HXD_BM][HXD_ACC_LD] accumulators of a half tile
+  float* ax = accs + HXD_BM * HXD_ACC_LD;                                         // [HXD_BH] row terms of that half tile
+  uint64_t* full = reinterpret_cast<uint64_t*>(ax + HXD_BH);                      // [HXD_STAGES] slot filled (TMA bytes landed)
+  uint64_t* empty = full + HXD_STAGES;                                            // [HXD_STAGES] slot read by every consumer warp
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-  const uint32_t rank = hxd_cta_rank();                     // 0 = leader (issues the MMAs of the pair)
-  const uint32_t pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
   if (threadIdx.x == 0) {
     hxd_prefetch_tmap(&map_q);
     hxd_prefetch_tmap(&map_x);
     for (int s = 0; s < HXD_STAGES; ++s) {
-      hx_mbar_init(full + s, 1);                             // the leader's producer: one arrive.expect_tx for both CTAs' bytes
-      hx_mbar_init(empty + s, 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      hx_mbar_init(tfull + s, 1);
-      hx_mbar_init(tempty + s, 2 * HXD_EPI_THREADS);
+      hx_mbar_init(full + s, 1);                       // the producer's arrive.expect_tx
+      hx_mbar_init(empty + s, HXD_CONSUMERS / 32);     // one arrive per consumer warp
     }
     hx_fence_mbar_init();
   }
-  if (warp == 2) hxd_tmem_alloc(tmem_slot, 512);
-  hxd_fence_before();
-  hxd_cluster_sync();       // barriers of both CTAs initialised before any remote arrive / complete_tx; TMEM allocated
-  hxd_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t total_units = a.m_pairs * a.n_split;
+  __syncthreads();
+  const uint32_t total_units = a.m_tiles * a.n_split;
 
-  if (warp == 0) {
-    // ===== TMA producer (one lane, in BOTH CTAs: own 128 queries + own half of the corpus tile) =====
+  if (warp == HXD_CONSUMERS / 32) {
+    // ===== TMA producer (one lane) =====
     if (lane == 0) {
       uint32_t stage = 0, ph = 0;
-      for (uint32_t u = pair; u < total_units; u += n_pairs) {
-        // units with the same n-range and different query pairs run on neighbouring CTA pairs in step: the corpus tile is
+      for (uint32_t u = blockIdx.x; u < total_units; u += gridDim.x) {
+        // units with the same n-range and different query tiles run on neighbouring CTAs in step: the corpus tile is
         // read from HBM once and served to the others by L2
-        const uint32_t mt = 2u * (u % a.m_pairs) + rank, r = u / a.m_pairs;
+        const uint32_t mt = u % a.m_tiles, r = u / a.m_tiles;
         const uint32_t nt0 = (uint32_t)((uint64_t)r * a.n_tiles / a.n_split), nt1 = (uint32_t)((uint64_t)(r + 1) * a.n_tiles / a.n_split);
         for (uint32_t nt = nt0; nt < nt1; ++nt)
-          for (uint32_t kb = 0; kb < a.k_blocks; ++kb) {
-            hx_mbar_wait(empty + stage, ph ^ 1u);           // own slot free (the multicast commit arrives in both CTAs)
-            unsigned char* sa = tiles + (size_t)stage * HXD_STAGE_BYTES;
-            const uint32_t lead_full = hxd_mapa(hx_smem_u32(full + stage), 0u);
-            if (rank == 0) hx_mbar_expect_tx(full + stage, 2u * HXD_STAGE_BYTES);
-            hxd_tma_load_2d(sa, &map_q, lead_full, (int)(kb * HXD_BK), (int)(mt * HXD_BM));
-            hxd_tma_load_2d(sa + HXD_A_BYTES, &map_x, lead_full, (int)(kb * HXD_BK), (int)(nt * HXD_BN + rank * (HXD_BN / 2)));
-            if (++stage == HXD_STAGES) { stage = 0; ph ^= 1u; }
-          }
+          for (uint32_t h = 0; h < HXD_BN / HXD_BH; ++h)
+            for (uint32_t kb = 0; kb < a.k_blocks; ++kb) {
+              hx_mbar_wait(empty + stage, ph ^ 1u);
+              unsigned char* sa = tiles + (size_t)stage * HXD_STAGE_BYTES;
+              hx_mbar_expect_tx(full + stage, HXD_STAGE_BYTES);
+              hxd_tma_load_2d(sa, &map_q, full + stage, (int)(kb * HXD_BK), (int)(mt * HXD_BM));
+              hxd_tma_load_2d(sa + HXD_A_BYTES, &map_x, full + stage, (int)(kb * HXD_BK), (int)(nt * HXD_BN + h * HXD_BH));
+              if (++stage == HXD_STAGES) { stage = 0; ph ^= 1u; }
+            }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one lane of the LEADER CTA, for the pair) =====
-    if (lane == 0 && rank == 0) {
-      // InstrDescriptor: c_format F32 (1<<4) | a_format BF16 (1<<7) | b_format BF16 (1<<10) | K-major A,B | N>>3 at 17 | M>>4 at 24
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(HXD_BN >> 3) << 17) | ((uint32_t)((2 * HXD_BM) >> 4) << 24);
-      uint32_t stage = 0, ph = 0, acc = 0, acc_ph = 0;
-      for (uint32_t u = pair; u < total_units; u += n_pairs) {
-       const uint32_t r = u / a.m_pairs;
-       const uint32_t nt0 = (uint32_t)((uint64_t)r * a.n_tiles / a.n_split), nt1 = (uint32_t)((uint64_t)(r + 1) * a.n_tiles / a.n_split);
-       for (uint32_t nt = nt0; nt < nt1; ++nt) {
-        hx_mbar_wait(tempty + acc, acc_ph ^ 1u);   // both epilogues have drained this accumulator stage
-        hxd_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * HXD_BN;
+    return;
+  }
+
+  // ===== consumers: warpgroup wg issues the MMAs of queries 64*wg .. 64*wg+63; all 256 threads run the epilogue =====
+  const uint32_t wg = warp >> 2;
+  const uint32_t erow = threadIdx.x & (HXD_BM - 1u);   // epilogue: query row of the tile ...
+  const uint32_t eq = threadIdx.x / HXD_BM;            // ... and 64-column quarter within the half tile
+  uint32_t stage = 0, ph = 0;
+  for (uint32_t u = blockIdx.x; u < total_units; u += gridDim.x) {
+    const uint32_t mt = u % a.m_tiles, r = u / a.m_tiles;
+    const uint32_t nt0 = (uint32_t)((uint64_t)r * a.n_tiles / a.n_split), nt1 = (uint32_t)((uint64_t)(r + 1) * a.n_tiles / a.n_split);
+    const uint32_t qrow = mt * HXD_BM + erow;
+    const float qa = qrow < a.n_queries ? a.q_aux[qrow] : 0.f;
+    // running best-T (largest t) of this query over the run, for quarter eq (first half) and quarter 2 + eq (second half);
+    // t = s*ax (cosine) or 2s - ax (euclidean)
+    float bt0[HXD_T], bt1[HXD_T];
+    uint32_t bs0[HXD_T], bs1[HXD_T];
+#pragma unroll
+    for (int i = 0; i < HXD_T; ++i) {
+      bt0[i] = bt1[i] = -__int_as_float(0x7f800000);
+      bs0[i] = bs1[i] = HX_ABSENT;
+    }
+    for (uint32_t nt = nt0; nt < nt1; ++nt) {
+      const uint32_t n0 = nt * HXD_BN;
+      for (uint32_t h = 0; h < HXD_BN / HXD_BH; ++h) {
+        float d[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) d[i] = 0.f;
+        uint32_t prev = 0;
         for (uint32_t kb = 0; kb < a.k_blocks; ++kb) {
-          hx_mbar_wait(full + stage, ph);          // both CTAs' tiles have landed
-          hxd_fence_after();
+          hx_mbar_wait(full + stage, ph);
           const uint32_t sa = hx_smem_u32(tiles + (size_t)stage * HXD_STAGE_BYTES);
-          const uint64_t adesc = hxd_make_desc(sa), bdesc = hxd_make_desc(sa + HXD_A_BYTES);
+          const uint64_t adesc = hxd_make_desc(sa + wg * (HXD_A_BYTES / 2)), bdesc = hxd_make_desc(sa + HXD_A_BYTES);
+          hxd_wgmma_fence();
 #pragma unroll
           for (uint32_t k = 0; k < HXD_BK / 16; ++k)   // 16 bf16 = 32 bytes along K inside the swizzle atom: start address += 2
-            hxd_umma(tmem_d, adesc + 2ull * k, bdesc + 2ull * k, idesc, (kb | k) ? 1u : 0u);
-          hxd_umma_commit_pair(empty + stage);        // slot reusable in both CTAs once these MMAs have read it
+            hxd_wgmma(d, adesc + 2ull * k, bdesc + 2ull * k, (kb | k) ? 1u : 0u);
+          hxd_wgmma_commit();
+          hxd_wgmma_wait<1>();                       // the group of k-block kb-1 has completed: its slot is free
+          if (kb > 0 && lane == 0) hx_mbar_arrive(empty + prev);
+          prev = stage;
           if (++stage == HXD_STAGES) { stage = 0; ph ^= 1u; }
         }
-        hxd_umma_commit_pair(tfull + acc);            // accumulator complete (each CTA drains its own 128 lanes)
-        if (++acc == 2) { acc = 0; acc_ph ^= 1u; }
-       }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: 16 warps; thread = one query row x one quarter (64 columns) of the tile =====
-    // A warp's column work is ONE dependent instruction stream (a lane is a query; whenever any of the 32 admits a column the
-    // warp walks the staging path).  With 8 warps x 128 columns that stream took longer per tile than the tile's 12 k-blocks
-    // of MMAs (profiles/r02_dense_limiter_experiments.json: the epilogue's column work cost 0.36 ms of a 1.6 ms kernel and
-    // 4 extra instructions per 8 columns cost another 0.28 ms): 16 warps x 64 columns halve it.
-    // ncu on the first version (profiles/): the tensor pipe sat at 10 % because 4 warps x 256 columns x ~30 instructions
-    // per column could not drain an accumulator as fast as the MMAs filled it.  Now the test is done in the dot-product
-    // domain (one FMUL/FFMA + one compare per column: the score is monotone in it), padded rows carry a sentinel that
-    // can never pass, row terms are read as float4, and two warps share each TMEM lane quarter.
-    const uint32_t ew = warp - 4;                     // 0..15
-    const uint32_t q4 = ew & 3u;                      // TMEM lane quarter this warp may access (warp id % 4)
-    const uint32_t half = ew >> 2;                    // column quarter 0..3
-    const uint32_t row_in_tile = q4 * 32 + lane;
-    const uint32_t et = threadIdx.x - 128;            // 0..511
-    uint32_t acc = 0, acc_ph = 0;
-    const uint32_t lead_tempty0 = hxd_mapa(hx_smem_u32(tempty), 0u);
-    for (uint32_t u = pair; u < total_units; u += n_pairs) {
-      const uint32_t mt = 2u * (u % a.m_pairs) + rank, r = u / a.m_pairs;
-      const uint32_t nt0 = (uint32_t)((uint64_t)r * a.n_tiles / a.n_split), nt1 = (uint32_t)((uint64_t)(r + 1) * a.n_tiles / a.n_split);
-      const uint32_t qrow = mt * HXD_BM + row_in_tile;
-      const float qa = qrow < a.n_queries ? a.q_aux[qrow] : 0.f;
-      // running best-T (largest t) of this query over the whole run of tiles; t = s*ax (cosine) or 2s - ax (euclidean)
-      float bt[HXD_T];
-      uint32_t bs[HXD_T];
+        hxd_wgmma_wait<0>();
+        hxd_fence_acc(d);
+        if (lane == 0) hx_mbar_arrive(empty + prev);
+        {   // accumulators -> shared memory (layout of hxd_wgmma), row terms of the half tile
+          float* p0 = accs + (64u * wg + 16u * (warp & 3u) + (lane >> 2)) * HXD_ACC_LD + 2u * (lane & 3u);
+          float* p1 = p0 + 8 * HXD_ACC_LD;
 #pragma unroll
-      for (int i = 0; i < HXD_T; ++i) { bt[i] = -__int_as_float(0x7f800000); bs[i] = HX_ABSENT; }
-      float thr = -__int_as_float(0x7f800000);
-      uint32_t cnt = 0;
-      for (uint32_t nt = nt0; nt < nt1; ++nt) {
-        const uint32_t n0 = nt * HXD_BN;
-        float* ax = aux + acc * HXD_BN;
-        {
-          const uint32_t c = et;                        // the first 256 threads stage the 256 row terms of the tile
-          if (c < HXD_BN) {
-            const bool live = n0 + hxd_row_at_pos(c) < a.n_rows;   // row_aux is indexed by POSITION, the bound is on the row there
-            float v = live ? a.row_aux[n0 + c] : 0.f;
+          for (int j = 0; j < 16; ++j) {
+            p0[8 * j] = d[4 * j]; p0[8 * j + 1] = d[4 * j + 1];
+            p1[8 * j] = d[4 * j + 2]; p1[8 * j + 1] = d[4 * j + 3];
+          }
+          const uint32_t c = threadIdx.x;
+          if (c < HXD_BH) {
+            const uint32_t pos = h * HXD_BH + c;
+            const bool live = n0 + hxd_row_at_pos(pos) < a.n_rows;   // row_aux is indexed by POSITION, the bound is on the row there
+            float v = live ? a.row_aux[n0 + pos] : 0.f;
             if (!live) v = a.metric == HXM_COSINE ? -__int_as_float(0x7f800000) : __int_as_float(0x7f800000);
             ax[c] = v;                                  // padded rows: t = NaN / -inf never beats the threshold
           }
         }
-        asm volatile("bar.sync 1, 512;" ::: "memory");
-        hx_mbar_wait(tfull + acc, acc_ph);
-        hxd_fence_after();
-        const uint32_t taddr = tmem_base + ((q4 * 32u) << 16) + acc * HXD_BN + half * (HXD_BN / HXD_PARTS);
-        const float4* ax4 = reinterpret_cast<const float4*>(ax + half * (HXD_BN / HXD_PARTS));
-        const uint32_t slot0 = n0 + half * (HXD_BN / HXD_PARTS);
-        // The loop body is deliberately small and NOT unrolled: the first version inlined the insertion network at every
-        // column (10k SASS instructions, instruction-cache bound: tensor pipe 9 %).  Columns that beat the running
-        // threshold are only STAGED (two predicated shared-memory stores); the single insertion-network instance below
-        // drains the staging area.
-        // round 2: the accumulator is read 32 columns at a time and DOUBLE BUFFERED — the tcgen05.ld of chunk i+1 is in
-        // flight while chunk i is tested — instead of sixteen serialised x8 loads per half tile: with two epilogue warps
-        // per scheduler the TMEM round trip (not the instruction count) was what kept the tensor pipe at 54 % (ncu,
-        // profiles/r02_ncu_dense_v1_raw.txt)
-        auto drain = [&]() {   // the insertion network (one instance per call site: eight in all)
-#pragma unroll 1
-          for (uint32_t i = 0; i < cnt; ++i) {
-            const float tvi = stg_t[i * HXD_EPI_THREADS + et];
-            if (tvi > bt[HXD_T - 1]) {
-              bt[HXD_T - 1] = tvi;
-              bs[HXD_T - 1] = stg_s[i * HXD_EPI_THREADS + et];
-#pragma unroll
-              for (int j = HXD_T - 1; j > 0; --j)
-                if (bt[j] > bt[j - 1]) {
-                  const float tf = bt[j]; bt[j] = bt[j - 1]; bt[j - 1] = tf;
-                  const uint32_t tsl = bs[j]; bs[j] = bs[j - 1]; bs[j - 1] = tsl;
-                }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        {
+          const uint32_t part = h * (HXD_BH / 64) + eq;   // column quarter of the placement tile
+          const float* rowp = accs + erow * HXD_ACC_LD + eq * 64u;
+          const float* axp = ax + eq * 64u;
+          // one instance of the insertion network per bucket: the loop is kept rolled (instruction cache)
+          auto scan = [&](float (&bt)[HXD_T], uint32_t (&bs)[HXD_T]) {
+#pragma unroll 4
+            for (uint32_t c = 0; c < 64; ++c) {
+              const float s = rowp[c], x = axp[c];
+              const float t = a.metric == HXM_COSINE ? s * x : fmaf(2.0f, s, -x);
+              if (t > bt[HXD_T - 1]) hxd_insert(bt, bs, t, n0 + hxd_row_at_pos(part * 64u + c));
             }
-          }
-          cnt = 0;
-          thr = bt[HXD_T - 1];
-        };
-        auto test8 = [&](const uint32_t* rr, uint32_t c0, bool last) {   // eight columns against the running threshold
-          const float4 x0 = ax4[(c0 >> 2)], x1 = ax4[(c0 >> 2) + 1];
-          float tv[8];
-          if (a.metric == HXM_COSINE) {
-            tv[0] = __uint_as_float(rr[0]) * x0.x; tv[1] = __uint_as_float(rr[1]) * x0.y;
-            tv[2] = __uint_as_float(rr[2]) * x0.z; tv[3] = __uint_as_float(rr[3]) * x0.w;
-            tv[4] = __uint_as_float(rr[4]) * x1.x; tv[5] = __uint_as_float(rr[5]) * x1.y;
-            tv[6] = __uint_as_float(rr[6]) * x1.z; tv[7] = __uint_as_float(rr[7]) * x1.w;
-          } else {
-            tv[0] = fmaf(2.0f, __uint_as_float(rr[0]), -x0.x); tv[1] = fmaf(2.0f, __uint_as_float(rr[1]), -x0.y);
-            tv[2] = fmaf(2.0f, __uint_as_float(rr[2]), -x0.z); tv[3] = fmaf(2.0f, __uint_as_float(rr[3]), -x0.w);
-            tv[4] = fmaf(2.0f, __uint_as_float(rr[4]), -x1.x); tv[5] = fmaf(2.0f, __uint_as_float(rr[5]), -x1.y);
-            tv[6] = fmaf(2.0f, __uint_as_float(rr[6]), -x1.z); tv[7] = fmaf(2.0f, __uint_as_float(rr[7]), -x1.w);
-          }
-#pragma unroll
-          for (int e = 0; e < 8; ++e)
-            if (tv[e] > thr) {
-              stg_t[cnt * HXD_EPI_THREADS + et] = tv[e];
-#if HXD_INTERLEAVE
-              stg_s[cnt * HXD_EPI_THREADS + et] = n0 + (c0 + e) * HXD_PARTS + half;   // hxd_row_at_pos(half * 64 + c0 + e)
-#else
-              stg_s[cnt * HXD_EPI_THREADS + et] = slot0 + c0 + e;
-#endif
-              ++cnt;
-            }
-          if (cnt > HXD_STAGE_CAP - 8 || last) drain();
-        };
-        {   // 64 columns: two 32-column loads, the second in flight while the first is tested (16-column halves of `rb`
-            // would save registers, but 640 threads leave 96 each and this fits)
-          uint32_t ra[32], rb[32];
-          hxd_tmem_ld32_nowait(taddr, ra);
-          hxd_tmem_wait_ld();
-          hxd_tmem_ld32_nowait(taddr + 32, rb);
-          test8(ra, 0, false); test8(ra + 8, 8, false); test8(ra + 16, 16, false); test8(ra + 24, 24, false);
-          hxd_tmem_wait_ld();
-          test8(rb, 32, false); test8(rb + 8, 40, false); test8(rb + 16, 48, false); test8(rb + 24, 56, true);
+          };
+          if (h == 0) scan(bt0, bs0);
+          else scan(bt1, bs1);
         }
-        hxd_fence_before();
-        hxd_mbar_arrive_cluster(lead_tempty0 + acc * 8u);   // 2 x 256 arrivals (both CTAs) free the accumulator stage
-        if (++acc == 2) { acc = 0; acc_ph ^= 1u; }
+        asm volatile("bar.sync 1, 256;" ::: "memory");   // the accumulator tile is free for the next half
       }
-      if (qrow < a.n_queries) {
-        uint64_t* out = a.keys + (((size_t)qrow * a.n_split + r) * HXD_PARTS + half) * HXD_T;
+    }
+    if (qrow < a.n_queries) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const uint32_t part = hh * (HXD_BH / 64) + eq;
+        uint64_t* out = a.keys + (((size_t)qrow * a.n_split + r) * HXD_PARTS + part) * HXD_T;
 #pragma unroll
         for (int i = 0; i < HXD_T; ++i) {
+          const float t = hh ? bt1[i] : bt0[i];
+          const uint32_t s = hh ? bs1[i] : bs0[i];
           uint64_t key = HX_KEY_MAX;
-          if (bs[i] != HX_ABSENT) {
-            float sc = a.metric == HXM_COSINE ? 0.5f - 0.5f * bt[i] * qa : qa - bt[i];   // (1-cos)/2 ; |q|^2 + |x|^2 - 2<q,x>
+          if (s != HX_ABSENT) {
+            float sc = a.metric == HXM_COSINE ? 0.5f - 0.5f * t * qa : qa - t;   // (1-cos)/2 ; |q|^2 + |x|^2 - 2<q,x>
             sc = fmaxf(sc, 0.0f);
-            key = hx_make_key(sc, bs[i]);
+            key = hx_make_key(sc, s);
           }
           out[i] = key;
         }
       }
     }
   }
-  hxd_fence_before();
-  hxd_cluster_sync();       // the leader's MMAs wrote BOTH CTAs' TMEM: nobody frees before both are done
-  if (warp == 2) hxd_tmem_dealloc(tmem_base, 512);
 }
 
 // f32 rows -> bf16 rows (round to nearest even) with zero padding to ldb, plus the per-row aux term computed from the
@@ -540,20 +414,19 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
   const uint32_t ldb = (dim + HXD_BK - 1) / HXD_BK * HXD_BK;
   if ((rc = ensure_bf16(ix, ldb))) return rc;
   const size_t n = ix->n;
-  const uint32_t m_pairs = (uint32_t)((B + 2 * HXD_BM - 1) / (2 * HXD_BM)), n_tiles = (uint32_t)((n + HXD_BN - 1) / HXD_BN);
-  const size_t B_pad = (size_t)m_pairs * 2 * HXD_BM, n_pad = (size_t)n_tiles * HXD_BN;
-  const size_t n_cta_pairs = (size_t)std::max(1, ix->sm_count / 2);   // one persistent CTA pair per TPC
+  const uint32_t m_tiles = (uint32_t)((B + HXD_BM - 1) / HXD_BM), n_tiles = (uint32_t)((n + HXD_BN - 1) / HXD_BN);
+  const size_t B_pad = (size_t)m_tiles * HXD_BM, n_pad = (size_t)n_tiles * HXD_BN;
+  const size_t n_ctas = (size_t)std::max(1, ix->sm_count);   // one persistent CTA per SM
   const uint32_t kprime = (uint32_t)std::min<size_t>(std::max<uint32_t>(4 * k, 64), std::min<size_t>(800, n));
-  // runs per query pair: enough units to fill the CTA pairs, and enough that one run's best-T comfortably covers its share
+  // runs per query tile: enough units to fill the CTAs, and enough that one run's best-T comfortably covers its share
   // of the k' nominees even when the true neighbours cluster in id space (8x head-room)
   uint32_t n_split = (uint32_t)std::max<size_t>(1, std::min<size_t>(n_tiles,
-      std::max<size_t>(std::max<size_t>(4, n_cta_pairs / m_pairs), (8 * (size_t)kprime + HXD_PARTS * HXD_T - 1) / (HXD_PARTS * HXD_T))));
-  // the grid is one persistent CTA pair per TPC: make the number of work units a multiple of it so that the last wave is
-  // full (1024 queries = 4 query pairs: 32 runs = 128 units = 1.73 waves of 74 pairs, the tensor pipe idles 13 % of the
-  // launch; 37 runs = 148 units = exactly 2 waves)
-  if ((size_t)m_pairs * n_split > n_cta_pairs)
+      std::max<size_t>(std::max<size_t>(4, n_ctas / m_tiles), (8 * (size_t)kprime + HXD_PARTS * HXD_T - 1) / (HXD_PARTS * HXD_T))));
+  // the grid is one persistent CTA per SM: make the number of work units a multiple of it so that the last wave is full
+  // (1024 queries = 8 query tiles: 32 runs = 256 units = 1.94 waves of 132 CTAs; 33 runs = 264 units = exactly 2 waves)
+  if ((size_t)m_tiles * n_split > n_ctas)
     for (uint32_t cand = n_split; cand <= std::min<uint32_t>(n_tiles, 2 * n_split); ++cand)
-      if (((size_t)m_pairs * cand) % n_cta_pairs == 0) { n_split = cand; break; }
+      if (((size_t)m_tiles * cand) % n_ctas == 0) { n_split = cand; break; }
   const size_t nkeys = B * (size_t)n_split * HXD_PARTS * HXD_T;
   int mi = 0;
   bool grew = false;
@@ -593,7 +466,7 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
     dc.ldb = ldb;
   }
   if (dc.map_x_base != ix->d_vec_bf16 || dc.map_x_rows != n_pad) {
-    if ((rc = make_map(reinterpret_cast<CUtensorMap*>(dc.map_x), ix->d_vec_bf16, n_pad, ldb, HXD_BN / 2))) return rc;   // a CTA stages half a corpus tile
+    if ((rc = make_map(reinterpret_cast<CUtensorMap*>(dc.map_x), ix->d_vec_bf16, n_pad, ldb, HXD_BH))) return rc;   // one MMA tile = half a placement tile
     dc.map_x_base = ix->d_vec_bf16;
     dc.map_x_rows = n_pad;
   }
@@ -617,20 +490,20 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
   a.n_rows = (uint32_t)n;
   a.n_queries = (uint32_t)B;
   a.k_blocks = ldb / HXD_BK;
-  a.m_pairs = m_pairs;
+  a.m_tiles = m_tiles;
   a.n_tiles = n_tiles;
   a.n_split = n_split;
   a.row_aux = ix->d_sqnorm;
   a.q_aux = d_qaux;
   a.keys = d_keys;
   a.metric = ix->cfg.metric;
-  const size_t smem = (size_t)HXD_STAGES * HXD_STAGE_BYTES + 16 * 8 + 16 + 2 * HXD_BN * 4 + (size_t)HXD_STAGE_CAP * HXD_EPI_THREADS * 8 + 1024;
+  const size_t smem = (size_t)HXD_STAGES * HXD_STAGE_BYTES + (size_t)HXD_BM * HXD_ACC_LD * 4 + HXD_BH * 4 + 2 * HXD_STAGES * 8 + 1024;
   static std::atomic<int> attr_set[64];
   if (!attr_set[ix->device & 63].load()) {
     HX_CUDA(cudaFuncSetAttribute(k_dense_scores, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set[ix->device & 63].store(1);
   }
-  const uint32_t grid = 2u * (uint32_t)std::min<size_t>((size_t)m_pairs * n_split, n_cta_pairs);   // clusters of 2 (__cluster_dims__)
+  const uint32_t grid = (uint32_t)std::min<size_t>((size_t)m_tiles * n_split, n_ctas);
   if (e0) HX_CUDA(cudaEventRecord(e0, stream));
   k_dense_scores<<<grid, HXD_THREADS, smem, stream>>>(*reinterpret_cast<CUtensorMap*>(dc.map_q),
                                                       *reinterpret_cast<CUtensorMap*>(dc.map_x), a);

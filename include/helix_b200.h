@@ -1,5 +1,5 @@
 /*
- * helix_b200.h — C ABI of the B200-native vector-search inner loop for HelixDB.
+ * helix_b200.h — C ABI of the CUDA (H100, sm_90a) vector-search inner loop for HelixDB.
  *
  * This is the drop-in boundary.  Every entry point is `extern "C"`, takes plain
  * pointers and sizes, returns an `hx_status` (0 = OK) and never throws or aborts.
@@ -468,7 +468,7 @@ hx_status hx_shard_group_last_ms(hx_shard_group* g, float* local_ms, float* coll
 
 /* ---- dense batched path (tensor cores; configs C4/C5) ---------------------------------- */
 /* Exhaustive top-k of B queries against all rows through the bf16 copy:
- * tcgen05 MMA for the B x N contraction, per-tile candidate filter, fp32 re-rank of
+ * wgmma (Hopper tensor cores) for the B x N contraction, per-tile candidate filter, fp32 re-rank of
  * survivors with the exact kernel.  Requires cfg.storage == 1. */
 hx_status hx_search_dense(hx_index* idx, const float* queries, size_t B, const hx_search_params* p,
                           uint64_t* out_ids, float* out_scores, uint32_t* out_counts,

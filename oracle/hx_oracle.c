@@ -7,7 +7,7 @@
  * never contracts a*b+c and never re-associates float sums; the only fused operations
  * are the explicit _mm256_fmadd_ps calls of spaces/simple_avx.rs.
  *
- * All "V/" paths are /root/reference/crates/db/src/search/vector/.
+ * All "V/" paths are helix-db/crates/db/src/search/vector/.
  */
 #define _GNU_SOURCE
 #include "hx_oracle.h"

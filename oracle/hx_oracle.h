@@ -4,7 +4,7 @@
  * TEST INFRASTRUCTURE ONLY.  This is the parity oracle and the CPU baseline of
  * bench.py; nothing in the product path (helix-db_b200/) may include, link or
  * call it.  Every function cites the reference file:line it restates (paths are
- * relative to /root/reference/crates/db/src/search/vector/).
+ * relative to helix-db/crates/db/src/search/vector/).
  *
  * Pinning: checked against the reference's own known-answer tests (SURVEY §8c,
  * tests/test_oracle_kat.py).  Strict-exhaustive search and the layer-0 policy functions are
@@ -191,7 +191,7 @@ int hxo_index_import_graph(hxo_index* idx, const uint16_t* levels, const uint32_
  * PARITY UNPINNED BY THE TREE: (1) the values drawn from the query session RNG — rand 0.10.2 `StdRng` = ChaCha12 seeded
  * through rand_core's `seed_from_u64` (PCG32 expansion), `random::<f32>()` = (next_u32 >> 8) * 2^-24,
  * `random_range(0..n)` = widening-multiply with one bias-correction draw — are restated from the published algorithms
- * of those crates (absent from /root/reference; no committed value pins them; the reference's own tests only compare
+ * of those crates (absent from the reference repository; no committed value pins them; the reference's own tests only compare
  * two instances of the generator).  What narrows that gap (tests/test_oracle_kat.py, vectors quoted from the published
  * crates' own value-stability tests, not from a file in the tree): the ChaCha12 stream — round count, counter / stream
  * start, word order, `from_rng` re-seeding — reproduces rand's `test_stdrng_construction` (10719222850664546238,

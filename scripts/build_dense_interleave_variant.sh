@@ -8,8 +8,8 @@ VAL="${1:-1}"
 TOPT="${2:-8}"
 TAG="il${VAL}"; [[ "$TOPT" != 8 ]] && TAG="il${VAL}_t${TOPT}"
 mkdir -p "$HERE/_variants"
-/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2,-Wall,-Wno-unused-function \
+/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2,-Wall,-Wno-unused-function \
   --fmad=false -DHXD_INTERLEAVE="$VAL" -DHXD_T="$TOPT" -Xptxas -v -c "$HERE/csrc/k_dense.cu" -o "$HERE/_variants/k_dense_$TAG.o"
-/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -shared -o "$HERE/_variants/libhelix_b200_$TAG.so" \
+/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -shared -o "$HERE/_variants/libhelix_b200_$TAG.so" \
   "$HERE/_obj/hx_api.o" "$HERE/_obj/k_build.o" "$HERE/_obj/hx_shard.o" "$HERE/_variants/k_dense_$TAG.o" -lcudart -ldl
 echo "built $HERE/_variants/libhelix_b200_$TAG.so"

@@ -45,5 +45,5 @@ for n in [int(x) for x in (sys.argv[1:] or ["20000", "100000"])]:
     print(json.dumps(res), flush=True)
     out.append(res)
     ix.close()
-(ROOT / "gpurun_out").mkdir(exist_ok=True)
-(ROOT / "gpurun_out" / "build_probe.json").write_text(json.dumps(out, indent=1))
+(ROOT / "scripts_out").mkdir(exist_ok=True)
+(ROOT / "scripts_out" / "build_probe.json").write_text(json.dumps(out, indent=1))

@@ -53,5 +53,5 @@ def one(n, recipe, sequential, nq=512):
 if __name__ == "__main__":
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 200_000
     out = [one(n, recipe, seq) for recipe in ("embedding", "survey") for seq in (False, True)]
-    (ROOT / "gpurun_out").mkdir(exist_ok=True)
-    (ROOT / "gpurun_out" / f"build_quality_{n}.json").write_text(json.dumps(out, indent=1))
+    (ROOT / "scripts_out").mkdir(exist_ok=True)
+    (ROOT / "scripts_out" / f"build_quality_{n}.json").write_text(json.dumps(out, indent=1))

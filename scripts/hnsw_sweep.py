@@ -2,7 +2,7 @@
 
 One index build, then for every variant (launch knobs of hx_tuning, given as their HX_* environment names and re-read with VectorIndex.tune()): warm-up, timed launches
 through hx_search_device, kernel time from the library's own CUDA events, algorithmic GB/s from the SearchStats counters,
-and a bit-for-bit comparison of ids/scores with the first variant.  Not the bench — writes gpurun_out/hnsw_sweep.json.
+and a bit-for-bit comparison of ids/scores with the first variant.  Not the bench — writes scripts_out/hnsw_sweep.json.
 
   python scripts/hnsw_sweep.py [--n 1000000] [--B 8192,16384] [--variants name=K:V,K:V;name2=...]
 """
@@ -85,8 +85,8 @@ def main():
                    "same_bits_as_first": same}
             print(json.dumps(run), flush=True)
             out["runs"].append(run)
-        (ROOT / "gpurun_out").mkdir(exist_ok=True)
-        (ROOT / "gpurun_out" / a.out).write_text(json.dumps(out, indent=1))
+        (ROOT / "scripts_out").mkdir(exist_ok=True)
+        (ROOT / "scripts_out" / a.out).write_text(json.dumps(out, indent=1))
         ix.close()
         return
     for B in [int(x) for x in a.B.split(",")]:
@@ -143,8 +143,8 @@ def main():
                 run["batch1_last_ids"] = o_ids[0].cpu().numpy().view(np.uint64).tolist()
             print(json.dumps(run), flush=True)
             out["runs"].append(run)
-    (ROOT / "gpurun_out").mkdir(exist_ok=True)
-    (ROOT / "gpurun_out" / a.out).write_text(json.dumps(out, indent=1))
+    (ROOT / "scripts_out").mkdir(exist_ok=True)
+    (ROOT / "scripts_out" / a.out).write_text(json.dumps(out, indent=1))
     ix.close()
 
 

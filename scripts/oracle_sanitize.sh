@@ -1,6 +1,6 @@
 #!/bin/bash
 # The CPU oracle (the parity checker) under AddressSanitizer + UBSan: its known-answer suite, the golden fixture and a
-# randomised mutation stress.  CPU only.  Log: profiles/r02_oracle_asan_ubsan.log
+# randomised mutation stress.  CPU only.
 set -euo pipefail
 ROOT="$(cd "$(dirname "${BASH_SOURCE[0]}")/.." && pwd)"
 cd "$ROOT"

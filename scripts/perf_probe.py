@@ -1,4 +1,4 @@
-"""Quick on-GPU probe (not the bench): scan GB/s and HNSW QPS at small/medium scale, written to gpurun_out/."""
+"""Quick on-GPU probe (not the bench): scan GB/s and HNSW QPS at small/medium scale, written to scripts_out/ (git-ignored)."""
 import json
 import sys
 import time
@@ -122,7 +122,7 @@ def hnsw_probe(n=20000, dim=768, B=4096, reps=3):
 
 
 if __name__ == "__main__":
-    Path(ROOT / "gpurun_out").mkdir(exist_ok=True)
+    Path(ROOT / "scripts_out").mkdir(exist_ok=True)
     which = sys.argv[1:] or ["scan", "hnsw"]
     if "scan" in which:
         for m in (hx.Metric.Euclidean, hx.Metric.Cosine):
@@ -131,4 +131,4 @@ if __name__ == "__main__":
     if "hnsw" in which:
         out["hnsw"] = hnsw_probe()
         print(json.dumps(out["hnsw"]), flush=True)
-    (ROOT / "gpurun_out" / "perf_probe.json").write_text(json.dumps(out, indent=1))
+    (ROOT / "scripts_out" / "perf_probe.json").write_text(json.dumps(out, indent=1))

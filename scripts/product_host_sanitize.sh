@@ -1,16 +1,16 @@
 #!/bin/bash
-# HOST code of the product library under AddressSanitizer + UBSan (device code untouched; compute-sanitizer covered that:
-# profiles/r02_sanitizer_*): builds helix-db_b200/_variants/libhelix_b200_asan.so, then runs the device-free ABI / codec /
-# host-logic tests and a byte-level fuzz of the row and key decoders on it.  CPU only.  Log: profiles/r02_product_host_asan_ubsan.log
+# HOST code of the product library under AddressSanitizer + UBSan (device code untouched): builds
+# helix-db_b200/_variants/libhelix_b200_asan.so, then runs the device-free ABI / codec / host-logic tests and a byte-level
+# fuzz of the row and key decoders on it.  CPU only.
 set -euo pipefail
 ROOT="$(cd "$(dirname "${BASH_SOURCE[0]}")/.." && pwd)"
 HERE="$ROOT/helix-db_b200"
 cd "$ROOT"
 mkdir -p "$HERE/_variants"
 [[ -f "$HERE/_obj/k_build.o" ]] || bash "$HERE/build.sh" > /dev/null
-/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -O1 -g -lineinfo -std=c++17 --fmad=false \
+/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -O1 -g -lineinfo -std=c++17 --fmad=false \
   -Xcompiler -fPIC,-O1,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -c "$HERE/csrc/hx_api.cu" -o "$HERE/_variants/hx_api_asan.o" 2> /dev/null
-/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -shared -Xcompiler -fsanitize=address,-fsanitize=undefined \
+/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -shared -Xcompiler -fsanitize=address,-fsanitize=undefined \
   -o "$HERE/_variants/libhelix_b200_asan.so" "$HERE/_variants/hx_api_asan.o" "$HERE/_obj/k_build.o" "$HERE/_obj/k_dense.o" "$HERE/_obj/hx_shard.o" -lcudart -ldl
 export HELIX_B200_LIB="$HERE/_variants/libhelix_b200_asan.so"
 export ASAN_OPTIONS=detect_leaks=0:abort_on_error=1:protect_shadow_gap=0

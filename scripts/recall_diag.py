@@ -38,5 +38,5 @@ out = []
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 1000000
 for kind, sigma in ((16, 0.5), (24, 0.5), (32, 0.5), (32, 1.0), (48, 0.7)):
     out.append(run(n, 1024, sigma, 0, tag=f"latent rank {kind} sigma {sigma}", kind=kind))
-(ROOT / "gpurun_out").mkdir(exist_ok=True)
-(ROOT / "gpurun_out" / "recall_diag_latent.json").write_text(json.dumps(out, indent=1))
+(ROOT / "scripts_out").mkdir(exist_ok=True)
+(ROOT / "scripts_out" / "recall_diag_latent.json").write_text(json.dumps(out, indent=1))

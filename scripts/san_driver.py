@@ -51,7 +51,7 @@ if "scan" in which:
     b = ix.search_restricted_batch(q[:10], hx.SearchParams.strict(40), cand)      # k_scan + k_select
     print("scan ok", int(a[2].sum()), int(b[2].sum()))
 if "dense" in which:
-    a = ix.search_dense_batch(q[:130], hx.SearchParams.strict(10))               # k_dense_scores (tcgen05) + re-rank
+    a = ix.search_dense_batch(q[:130], hx.SearchParams.strict(10))               # k_dense_scores (wgmma) + re-rank
     print("dense ok", int(a[2].sum()))
 if "service" in which:
     with ix.service(10, 40, capacity=64, max_batch=16) as svc:

@@ -58,7 +58,7 @@ int main() {
   CHECK(c.ids().size() == 2 && c.contains(3) && c.contains(7) && !c.contains(4) && !c.is_empty());
   CHECK(RestrictedVectorCandidates::from_ids({}).is_empty());
   CHECK(hx_order_code_from_simhash_bits(0) == 0 && hx_order_code_from_simhash_bits(1ull << 47) == 1ull << 62);
-  CHECK(std::strstr(hx_version(), "sm_100a") != nullptr);
+  CHECK(std::strstr(hx_version(), "sm_90a") != nullptr);
   CHECK(HelixDbError::variant(HX_ERR_ZERO_NORM_COSINE) == "ZeroNormCosineVector");
 
   // ---- the device: no CPU fallback ----

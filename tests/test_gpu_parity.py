@@ -660,7 +660,7 @@ def test_device_build(gm, om, n, dim, m):
     assert gi2["entry_point"] == 102 and gi2["max_layer"] == 3
 
 
-# ---- dense tensor-core path (tcgen05 bf16 contraction nominates, exact fp32 re-rank decides) -------------------------------------
+# ---- dense tensor-core path (wgmma bf16 contraction nominates, exact fp32 re-rank decides) -------------------------------------
 @pytest.mark.parametrize("gm,om,n,dim,B", [(hx.Metric.Cosine, hxo.COSINE, 5000, 768, 300),
                                           (hx.Metric.Euclidean, hxo.EUCLIDEAN, 3000, 100, 130),
                                           (hx.Metric.Cosine, hxo.COSINE, 700, 64, 5),

@@ -117,7 +117,7 @@ def _rank_main(rank, world, port, ret):
 def test_two_ranks_one_all_gather():
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two devices (gpurun --gpus 2)")
+        pytest.skip("needs two CUDA devices")
     import torch.multiprocessing as mp
     world, port = 2, _free_port()
     mgr = mp.Manager()

@@ -4,7 +4,7 @@ suite with `-x`, and everything above has a longer green history):
   * VectorIndex::delete (V/mutation.rs:1606-2050) restated in the oracle and applied to the device mirror as row patches,
     including a write that deletes the entry point and the whole top layer;
   * the C++ host mirror (helix-db_b200/host/vector_index.hpp) linked and executed: phase-0 KAT on the device.
-V/ = /root/reference/crates/db/src/search/vector/ (cited, never read at run time)."""
+V/ = helix-db/crates/db/src/search/vector/ (cited, never read at run time)."""
 import numpy as np
 import pytest
 
@@ -141,8 +141,7 @@ def test_cpp_host_mirror_runs_the_phase0_kat_on_the_device(tmp_path):
 def test_dense_path_keeps_id_clustered_neighbours(gm, om):
     """hx_search_dense nominates by bucket — (query, run of tiles, 64-column quarter), best HXD_T = 8 rows each.  With rows
     placed in id order a bucket holds 64 CONSECUTIVE ids per tile, so a query whose 11 nearest rows are consecutive ids (chunks
-    of one document inserted back to back) would keep only 8 of them (measured: recall 0.8 on exactly this fixture,
-    profiles/r02_dense_row_placement_ab.json).  The interleaved placement (HXD_INTERLEAVE, csrc/k_dense.cu) spreads consecutive
+    of one document inserted back to back) would keep only 8 of them (recall 0.8 on exactly this fixture).  The interleaved placement (HXD_INTERLEAVE, csrc/k_dense.cu) spreads consecutive
     ids over the four quarters: every true neighbour must come back, with the oracle's exact scan as the ground truth."""
     rng = np.random.default_rng(77)
     n, dim, k, nh = 40_000, 64, 10, 16

@@ -1,7 +1,7 @@
 """Pins the CPU oracle against the reference's own known-answer tests (SURVEY §8c items 1-9).
 
-Paths: V/ = /root/reference/crates/db/src/search/vector/, T/ = /root/reference/crates/db/tests/production_support/.
-Nothing here reads /root/reference at run time: the expected values are the literals the reference's tests assert.
+Paths: V/ = helix-db/crates/db/src/search/vector/, T/ = helix-db/crates/db/tests/production_support/.
+Nothing here reads the reference repository at run time: the expected values are the literals the reference's tests assert.
 """
 import math
 import struct
@@ -474,7 +474,7 @@ def test_session_rng_structure(hxo):
 def test_chacha12_stream_matches_the_rand_crates_value_stability_vectors(hxo):
     """The session RNG is `rand::rngs::StdRng` (randomness.rs:96-165) = ChaCha12 over a 32-byte seed, output consumed as
     little-endian words in block order.  The rand / rand_chacha crates are NOT in the tree (SURVEY 8c), so these known
-    answers are quoted from the published crates' own value-stability tests, not from a file under /root/reference:
+    answers are quoted from the published crates' own value-stability tests, not from a file of the reference repository:
       * rand `rngs/std.rs::test_stdrng_construction`: seed [1,0,0,0, 23,0,0,0, 200,1,0,0, 210,30,0,0, 0 x 16],
         `next_u64()` = 10719222850664546238, and a second StdRng seeded with the NEXT 32 bytes of that stream
         (`from_rng` = `fill_bytes(seed)`) gives `next_u64()` = 14064965282130556830;
