@@ -182,6 +182,8 @@ ABI_SYMBOLS = [
     "hx_candidates_destroy", "hx_candidates_len", "hx_search_restricted_sets",
     "hx_search_batch", "hx_device_flags", "hx_service_create", "hx_service_destroy", "hx_service_submit",
     "hx_service_poll", "hx_service_wait", "hx_service_search", "hx_service_get_stats",
+    "hx_restricted_service_create", "hx_service_submit_restricted", "hx_service_submit_restricted_set",
+    "hx_service_search_restricted", "hx_service_search_restricted_set",
     "hx_shard_unique_id", "hx_shard_group_create", "hx_shard_group_destroy", "hx_search_sharded_device",
     "hx_search_sharded", "hx_search_restricted_sharded", "hx_shard_group_last_ms",
     "hx_index_upsert_vectors", "hx_index_set_levels", "hx_index_upsert_neighbor_rows", "hx_index_delete_vectors",
@@ -315,6 +317,16 @@ def load_library():
     L.hx_service_search.argtypes = [vp, fp, u64p, fp, u32p]
     L.hx_service_get_stats.restype = C.c_int32
     L.hx_service_get_stats.argtypes = [vp, C.POINTER(ServiceStats)]
+    L.hx_restricted_service_create.restype = C.c_int32
+    L.hx_restricted_service_create.argtypes = [vp, C.POINTER(_ServiceConfig), C.c_uint64, C.POINTER(vp)]
+    L.hx_service_submit_restricted.restype = C.c_int32
+    L.hx_service_submit_restricted.argtypes = [vp, fp, u64p, sz, u64p]
+    L.hx_service_submit_restricted_set.restype = C.c_int32
+    L.hx_service_submit_restricted_set.argtypes = [vp, fp, vp, u64p]
+    L.hx_service_search_restricted.restype = C.c_int32
+    L.hx_service_search_restricted.argtypes = [vp, fp, u64p, sz, u64p, fp, u32p]
+    L.hx_service_search_restricted_set.restype = C.c_int32
+    L.hx_service_search_restricted_set.argtypes = [vp, fp, vp, u64p, fp, u32p]
     L.hx_filtered_budgets.restype = None
     L.hx_filtered_budgets.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.POINTER(FilteredBudgets)]
     L.hx_search_filtered_graph.restype = C.c_int32
@@ -846,6 +858,10 @@ class VectorIndex:
         """A query service on this index: concurrent one-query callers coalesced into shared launches."""
         return SearchService(self, k, ef, **kw)
 
+    def restricted_service(self, k: int, arena_ids: int = 0, **kw) -> "RestrictedSearchService":
+        """A restricted query service: concurrent one-query search_restricted callers coalesced into shared scans."""
+        return RestrictedSearchService(self, k, arena_ids, **kw)
+
     def search_restricted(self, query, params: SearchParams, allowed: RestrictedVectorCandidates):
         """VectorIndex::search_restricted (restricted.rs:466-479); exact for every |C| <= 1e6."""
         ids, sc, cnt = self.search_restricted_batch(np.asarray(query, dtype=np.float32).reshape(1, -1), params,
@@ -1044,6 +1060,48 @@ class SearchService:
         st = ServiceStats()
         _ck(self.L.hx_service_get_stats(self.h, C.byref(st)))
         return st.as_dict()
+
+
+class RestrictedSearchService(SearchService):
+    """hx_restricted_service_create: ValidatedVectorReadIndex::search_restricted's calling pattern (one query and one
+    candidate set per call from many concurrent tasks, read_index.rs:92-101) served by shared exact-scan launches.
+    ``allowed`` is a RestrictedVectorCandidates (ids copied at submit) or a DeviceCandidates (resident on the device; it
+    must stay open until the ticket's results are out).  Answers are bit-identical to search_restricted."""
+
+    def __init__(self, index: VectorIndex, k: int, arena_ids: int = 0, capacity: int = 0, max_batch: int = 0,
+                 n_streams: int = 0, min_batch: int = 0, batch_window_us: int = 0, flags: int = 0):
+        self.L, self.index, self.k = index.L, index, int(k)
+        cfg = _ServiceConfig(int(k), 0, capacity, max_batch, n_streams, 0, 0, 0, 0, min_batch, batch_window_us, flags)
+        h = C.c_void_p()
+        _ck(self.L.hx_restricted_service_create(index.h, C.byref(cfg), int(arena_ids), C.byref(h)))
+        self.h = h
+
+    def _query(self, query):
+        qa, qp = _f32(query)
+        if qa.size != self.index.dim:
+            raise HelixDbError(HX_ERR_INVALID_DIMENSION, f"invalid dimension: expected {self.index.dim}, got {qa.size}")
+        return qa, qp
+
+    def submit(self, query, allowed) -> int:
+        qa, qp = self._query(query)
+        t = C.c_uint64(0)
+        if isinstance(allowed, DeviceCandidates):
+            _ck(self.L.hx_service_submit_restricted_set(self.h, qp, allowed.h, C.byref(t)))
+        else:
+            ca, cp = _u64(allowed.ids)
+            _ck(self.L.hx_service_submit_restricted(self.h, qp, cp, ca.size, C.byref(t)))
+        return int(t.value)
+
+    def search(self, query, allowed):
+        qa, qp = self._query(query)
+        ids, sc, cnt = self._out()
+        op = (ids.ctypes.data_as(C.POINTER(C.c_uint64)), sc.ctypes.data_as(C.POINTER(C.c_float)), C.byref(cnt))
+        if isinstance(allowed, DeviceCandidates):
+            _ck(self.L.hx_service_search_restricted_set(self.h, qp, allowed.h, *op))
+        else:
+            ca, cp = _u64(allowed.ids)
+            _ck(self.L.hx_service_search_restricted(self.h, qp, cp, ca.size, *op))
+        return [SearchResult(ids[i], sc[i]) for i in range(int(cnt.value))]
 
 
 def merge_topk_device(device, d_all_ids, d_all_scores, d_all_counts, n_shards, B, k, d_out_ids, d_out_scores,

@@ -234,13 +234,14 @@ struct HxSelectArgs {
   const uint64_t* q_keyoff;
 };
 
-// bitonic sort of 2*HX_SEL_HALF keys in shared memory, ascending
+// bitonic sort of 2*HX_SEL_HALF keys in shared memory, ascending, by a block of THREADS threads
+template <uint32_t THREADS>
 __device__ __forceinline__ void hx_bitonic_sort_2048(uint64_t* s, uint32_t tid) {
   const uint32_t N = 2 * HX_SEL_HALF;
   for (uint32_t size = 2; size <= N; size <<= 1) {
     for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
       __syncthreads();
-      for (uint32_t p = tid; p < N / 2; p += HX_SEL_THREADS) {
+      for (uint32_t p = tid; p < N / 2; p += THREADS) {
         const uint32_t i = 2 * p - (p & (stride - 1));   // index of the lower element of the pair
         const uint32_t j = i + stride;
         const bool up = ((i & size) == 0);
@@ -250,6 +251,37 @@ __device__ __forceinline__ void hx_bitonic_sort_2048(uint64_t* s, uint32_t tid) 
     }
   }
   __syncthreads();
+}
+
+// The kk (<= HX_SEL_HALF) smallest of keys[0, n) into buf[0, kk), ascending; buf[kk..] holds larger keys or HX_KEY_MAX.
+// Threshold filter + bitonic merge in shared memory, run by the whole block (block-uniform call; buf = 2*HX_SEL_HALF
+// keys).  The keys are read from L2 (__ldcg): the service kernel selects over keys other CTAs of the same launch wrote.
+template <uint32_t THREADS>
+__device__ __forceinline__ void hx_select_keys(const uint64_t* keys, uint64_t n, uint32_t kk, uint64_t* buf, uint32_t* s_cnt,
+                                               uint64_t* s_thr, uint32_t tid) {
+  for (uint32_t i = tid; i < 2 * HX_SEL_HALF; i += THREADS) buf[i] = HX_KEY_MAX;
+  if (tid == 0) { *s_cnt = 0; *s_thr = HX_KEY_MAX; }
+  __syncthreads();
+  for (uint64_t b0 = 0; b0 < n; b0 += THREADS) {
+    const uint64_t r = b0 + tid;
+    if (r < n) {
+      const uint64_t key = __ldcg(keys + r);
+      if (key < *s_thr) {
+        const uint32_t p = atomicAdd(s_cnt, 1u);
+        buf[HX_SEL_HALF + p] = key;            // p < HX_SEL_HALF guaranteed by the flush rule below
+      }
+    }
+    __syncthreads();
+    const uint32_t filled = *s_cnt;   // snapshot between two barriers: no thread can bump s_cnt before all have read it
+    __syncthreads();
+    if (filled + THREADS > HX_SEL_HALF) {   // next step could overflow: merge now (block-uniform)
+      hx_bitonic_sort_2048<THREADS>(buf, tid);
+      for (uint32_t i = tid; i < HX_SEL_HALF; i += THREADS) buf[HX_SEL_HALF + i] = HX_KEY_MAX;
+      if (tid == 0) { *s_cnt = 0; *s_thr = buf[kk - 1]; }   // HX_KEY_MAX until kk keys are known
+      __syncthreads();
+    }
+  }
+  hx_bitonic_sort_2048<THREADS>(buf, tid);
 }
 
 static __global__ void __launch_bounds__(HX_SEL_THREADS) k_select(HxDev ix, HxSelectArgs a) {
@@ -266,29 +298,7 @@ static __global__ void __launch_bounds__(HX_SEL_THREADS) k_select(HxDev ix, HxSe
     }
     const uint64_t* keys = a.keys + (a.q_slots ? a.q_keyoff[q] : (a.shared_set ? (uint64_t)q * a.n_shared : base));
     const uint32_t kk = (uint64_t)a.k < n ? a.k : (uint32_t)n;   // k' = min(k, |C|)
-    for (uint32_t i = tid; i < 2 * HX_SEL_HALF; i += HX_SEL_THREADS) buf[i] = HX_KEY_MAX;
-    if (tid == 0) { s_cnt = 0; s_thr = HX_KEY_MAX; }
-    __syncthreads();
-    for (uint64_t b0 = 0; b0 < n; b0 += HX_SEL_THREADS) {
-      const uint64_t r = b0 + tid;
-      if (r < n) {
-        const uint64_t key = keys[r];
-        if (key < s_thr) {
-          const uint32_t p = atomicAdd(&s_cnt, 1u);
-          buf[HX_SEL_HALF + p] = key;            // p < HX_SEL_HALF guaranteed by the flush rule below
-        }
-      }
-      __syncthreads();
-      const uint32_t filled = s_cnt;   // snapshot between two barriers: no thread can bump s_cnt before all have read it
-      __syncthreads();
-      if (filled + HX_SEL_THREADS > HX_SEL_HALF) {   // next step could overflow: merge now (block-uniform)
-        hx_bitonic_sort_2048(buf, tid);
-        for (uint32_t i = tid; i < HX_SEL_HALF; i += HX_SEL_THREADS) buf[HX_SEL_HALF + i] = HX_KEY_MAX;
-        if (tid == 0) { s_cnt = 0; s_thr = buf[kk - 1]; }   // HX_KEY_MAX until kk keys are known
-        __syncthreads();
-      }
-    }
-    hx_bitonic_sort_2048(buf, tid);
+    hx_select_keys<HX_SEL_THREADS>(keys, n, kk, buf, &s_cnt, &s_thr, tid);
     // count valid (absent candidates carry HX_KEY_MAX and are never results)
     const uint32_t* slots = a.q_slots ? a.q_slots[q] : a.cand_slots + base;
     uint32_t cnt = 0;
@@ -313,12 +323,8 @@ static __global__ void __launch_bounds__(HX_SEL_THREADS) k_select(HxDev ix, HxSe
 }
 
 // ---- candidate id -> slot mapping (restricted.rs:615-659: ids without a vector row are skipped) ----------
-static __global__ void k_map_candidates(const uint64_t* __restrict__ ids_sorted, uint32_t n, const uint64_t* __restrict__ cand,
-                                 uint64_t n_cand, uint32_t* __restrict__ out_slots, int contiguous, uint64_t first_id,
-                                 const uint8_t* __restrict__ deleted) {
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_cand) return;
-  const uint64_t id = cand[i];
+__device__ __forceinline__ uint32_t hx_candidate_slot(const uint64_t* __restrict__ ids_sorted, uint32_t n, uint64_t id,
+                                                      int contiguous, uint64_t first_id, const uint8_t* __restrict__ deleted) {
   uint32_t slot = HX_ABSENT;
   if (contiguous) {
     if (id >= first_id && id - first_id < (uint64_t)n) slot = (uint32_t)(id - first_id);
@@ -331,5 +337,190 @@ static __global__ void k_map_candidates(const uint64_t* __restrict__ ids_sorted,
     if (lo < n && ids_sorted[lo] == id) slot = lo;
   }
   if (deleted && slot != HX_ABSENT && deleted[slot]) slot = HX_ABSENT;   // hx_index_delete_vectors: the row is gone
-  out_slots[i] = slot;
+  return slot;
+}
+
+static __global__ void k_map_candidates(const uint64_t* __restrict__ ids_sorted, uint32_t n, const uint64_t* __restrict__ cand,
+                                 uint64_t n_cand, uint32_t* __restrict__ out_slots, int contiguous, uint64_t first_id,
+                                 const uint8_t* __restrict__ deleted) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_cand) return;
+  out_slots[i] = hx_candidate_slot(ids_sorted, n, cand[i], contiguous, first_id, deleted);
+}
+
+// ---- restricted query service: one launch per coalesced batch of one-query callers (hx_service_submit_restricted) ---------
+// The grid is the batch's flattened work list: query q owns units [unit0[q], unit0[q+1]), one CTA per `chunk` candidates
+// (chunk >= 256, so the reference's exact-plan shape |C| <= 256 is one CTA: no ticket, no partial list).  A CTA stages the
+// query and its chunk's candidate slots in shared memory (list submissions: ids read from the pinned arena and mapped
+// with hx_candidate_slot; device sets: slots as stored), scores every present row with the bit-exact octet kernel (one
+// thread per row for Manhattan) and keys it score_bits<<32 | rank, exactly as k_scan does.
+//   k <= 32: warp lists (hx_topk_insert / hx_topk_merge32) as in k_scan_topk; a query of several units merges the
+//            per-CTA lists in its last CTA (self-resetting ticket).
+//   k >  32: keys go to scratch; the query's last CTA selects with hx_select_keys (k_select's logic).
+// The CTA that finishes a query writes ids / scores / count into the host-mapped result slot, __threadfence_system, then
+// the slot's done word 0x80000000 | flags (the hx_query_done protocol).
+#define HX_RSVC_MAX_BATCH 128       // queries per launch: the descriptor travels as the kernel parameter
+#define HX_RSVC_CHUNK_MIN 256
+#define HX_RSVC_CHUNK_MAX 2048
+
+struct HxRsvcQuery {
+  const void* cand;     // list: ascending uint64 ids; device set: uint32 slots (HX_ABSENT = no vector row)
+  uint32_t n;           // |C| (> 0)
+  uint32_t is_set;
+};
+
+struct HxRsvcArgs {
+  const float* queries;          // [B][dim]  (the pinned ring itself or its device copy)
+  const float* q_hdr;            // [B]
+  const uint8_t* deleted;
+  int contiguous;
+  uint64_t first_id;
+  uint32_t B, k, chunk;
+  uint64_t* partial;             // [units][HX_TOPK]    (k <= 32)
+  uint64_t* keys;                // [units * chunk]     (k > 32): query q's keys start at unit0[q] * chunk
+  uint32_t* tickets;             // [B] zero; self-resetting
+  uint32_t* qflags;              // [B] zero; self-resetting
+  uint64_t* out_ids;             // [B][k]  host-mapped result slots
+  float* out_scores;             // [B][k]
+  uint32_t* out_counts;          // [B]
+  uint32_t* done;                // [B]
+  uint32_t unit0[HX_RSVC_MAX_BATCH + 1];
+  HxRsvcQuery q[HX_RSVC_MAX_BATCH];
+};
+
+template <int METRIC, bool BIGK>
+static __global__ void __launch_bounds__(HX_SCAN_THREADS, 4) k_scan_service(HxDev ix, const __grid_constant__ HxRsvcArgs a) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  float* sq = reinterpret_cast<float*>(smem);
+  __shared__ uint32_t s_slots[HX_RSVC_CHUNK_MAX];
+  __shared__ uint64_t s_lists[HX_SCAN_THREADS / 32][HX_TOPK];
+  __shared__ uint64_t s_buf[BIGK ? 2 * HX_SEL_HALF : 1];
+  __shared__ uint64_t s_thr;
+  __shared__ uint32_t s_cnt, s_last, s_flags;
+  const uint32_t tid = threadIdx.x, t = tid & 7u, oct = tid >> 3, lane = tid & 31u, warp = tid >> 5;
+  const unsigned FULL = 0xffffffffu;
+  const uint32_t unit = blockIdx.x;
+  // the owning query: the last q with unit0[q] <= unit (a query without units shares unit0 with its successor)
+  uint32_t q = 0, hi = a.B;
+  while (hi - q > 1) {
+    const uint32_t mid = (q + hi) >> 1;
+    if (a.unit0[mid] <= unit) q = mid; else hi = mid;
+  }
+  const HxRsvcQuery Q = a.q[q];
+  const uint32_t n = Q.n, first = a.unit0[q], nunits = a.unit0[q + 1] - first;
+  const uint32_t start = (unit - first) * a.chunk, end = min(start + a.chunk, n);
+  for (uint32_t i = tid; i < ix.ld; i += HX_SCAN_THREADS) sq[i] = i < ix.dim ? a.queries[(size_t)q * ix.dim + i] : 0.0f;
+  for (uint32_t r = start + tid; r < end; r += HX_SCAN_THREADS)
+    s_slots[r - start] = Q.is_set ? static_cast<const uint32_t*>(Q.cand)[r]
+                                  : hx_candidate_slot(ix.ids, ix.n, static_cast<const uint64_t*>(Q.cand)[r], a.contiguous,
+                                                      a.first_id, a.deleted);
+  if (tid == 0) s_flags = 0u;
+  const float q_hdr = a.q_hdr[q];
+  __syncthreads();
+  // scan: octets own rows (4 per warp per step), Manhattan one row per thread (32 per warp per step)
+  const uint32_t step = METRIC == HXM_MANHATTAN ? HX_SCAN_THREADS : HX_SCAN_THREADS / 8;
+  uint64_t mine = HX_KEY_MAX;
+  uint32_t flags = 0u;
+  for (uint32_t r0 = start; r0 < end; r0 += step) {
+    const uint32_t r = r0 + (METRIC == HXM_MANHATTAN ? tid : oct);
+    uint64_t key = HX_KEY_MAX;
+    if (r < end) {
+      const uint32_t slot = s_slots[r - start];
+      if (slot != HX_ABSENT) {
+        float s;
+        if (METRIC == HXM_MANHATTAN) s = hx_manhattan_seq(ix.vec + (size_t)slot * ix.ld, sq, ix.dim);
+        else s = hx_octet_score<METRIC>(ix, sq, q_hdr, slot, t);
+        if (!hx_score_ok(s)) flags |= HXF_INVALID_SCORE;
+        key = hx_make_key(s, r);
+      }
+    }
+    if (BIGK) {
+      if (r < end && (METRIC == HXM_MANHATTAN || t == 0)) a.keys[(size_t)first * a.chunk + r] = key;
+    } else {
+      uint64_t kth = __shfl_sync(FULL, mine, HX_TOPK - 1);
+      constexpr int PER_WARP = METRIC == HXM_MANHATTAN ? 32 : 4;
+#pragma unroll 4
+      for (int o = 0; o < PER_WARP; ++o) {
+        const uint64_t c = __shfl_sync(FULL, key, METRIC == HXM_MANHATTAN ? o : o * 8);
+        if (c < kth) {   // warp-uniform branch (c and kth are broadcasts)
+          hx_topk_insert(mine, c, lane);
+          kth = __shfl_sync(FULL, mine, HX_TOPK - 1);
+        }
+      }
+    }
+  }
+  if (flags) atomicOr(&s_flags, flags);
+  if (!BIGK) s_lists[warp][lane] = mine;
+  __syncthreads();
+  if (!BIGK && warp == 0) {
+#pragma unroll
+    for (uint32_t w = 1; w < HX_SCAN_THREADS / 32; ++w) mine = hx_topk_merge32(mine, s_lists[w][lane], lane);
+  }
+  uint32_t qf = s_flags;
+  if (nunits > 1) {   // publish this CTA's part; the last CTA of the query finishes it
+    if (!BIGK && warp == 0) a.partial[(size_t)unit * HX_TOPK + lane] = mine;
+    if (tid == 0 && qf) atomicOr(a.qflags + q, qf);
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(a.tickets + q, 1u) == nunits - 1u ? 1u : 0u;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    qf = __ldcg(a.qflags + q);
+    if (!BIGK) {   // warp w merges units w, w + 8, ... of the query
+      uint64_t best = HX_KEY_MAX;
+      for (uint32_t u = first + warp; u < first + nunits; u += HX_SCAN_THREADS / 32)
+        best = hx_topk_merge32(best, __ldcg(a.partial + (size_t)u * HX_TOPK + lane), lane);
+      s_lists[warp][lane] = best;
+      __syncthreads();
+      if (warp == 0) {
+        mine = best;
+#pragma unroll
+        for (uint32_t w = 1; w < HX_SCAN_THREADS / 32; ++w) mine = hx_topk_merge32(mine, s_lists[w][lane], lane);
+      }
+    }
+    __syncthreads();
+    if (tid == 0) { a.tickets[q] = 0u; a.qflags[q] = 0u; }   // ready for the next launch on this scratch
+  }
+  const uint32_t kk = a.k < n ? a.k : n;   // k' = min(k, |C|)
+  uint32_t cnt = 0;
+  auto result_id = [&](uint32_t rank) -> uint64_t {
+    return Q.is_set ? ix.ids[static_cast<const uint32_t*>(Q.cand)[rank]] : static_cast<const uint64_t*>(Q.cand)[rank];
+  };
+  if (!BIGK) {
+    if (warp != 0) return;
+    const bool have = lane < kk && mine != HX_KEY_MAX;
+    if (have) {
+      a.out_ids[(size_t)q * a.k + lane] = result_id((uint32_t)(mine & 0xffffffffu));
+      a.out_scores[(size_t)q * a.k + lane] = hx_key_score(mine);
+    }
+    cnt = __popc(__ballot_sync(FULL, have));
+    __threadfence_system();   // results before the done word
+    __syncwarp();
+    if (lane == 0) {
+      a.out_counts[q] = cnt;
+      __threadfence_system();
+      *((volatile uint32_t*)a.done + q) = 0x80000000u | qf;
+    }
+    return;
+  }
+  hx_select_keys<HX_SCAN_THREADS>(a.keys + (size_t)first * a.chunk, n, kk, s_buf, &s_cnt, &s_thr, tid);
+  for (uint32_t i = tid; i < kk; i += HX_SCAN_THREADS) {
+    const uint64_t key = s_buf[i];
+    if (key != HX_KEY_MAX) {
+      a.out_ids[(size_t)q * a.k + i] = result_id((uint32_t)(key & 0xffffffffu));
+      a.out_scores[(size_t)q * a.k + i] = hx_key_score(key);
+      cnt++;
+    }
+  }
+  if (tid == 0) s_cnt = 0u;
+  __syncthreads();
+  if (cnt) atomicAdd(&s_cnt, cnt);
+  __threadfence_system();
+  __syncthreads();
+  if (tid == 0) {
+    a.out_counts[q] = s_cnt;
+    __threadfence_system();
+    *((volatile uint32_t*)a.done + q) = 0x80000000u | qf;
+  }
 }

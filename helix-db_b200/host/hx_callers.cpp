@@ -9,10 +9,13 @@
 //                      submit() / poll()  (what a tokio worker does with the tasks it owns)
 //   mode 2  direct   : n_callers OS threads, each one blocking B = 1 hx_search call per query (no service: the
 //                      round-1 path, kept as the comparison)
+// hx_callers_run_restricted plays search_restricted the same way (one query + its candidate set per call); its direct
+// mode is one blocking B = 1 hx_search_restricted per call.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <cstring>
+#include <functional>
 #include <thread>
 #include <vector>
 
@@ -26,12 +29,17 @@ typedef struct {
   uint64_t completed, errors;
 } hx_callers_report;
 
-// queries: n_queries x dim.  Caller c walks queries c, c + n_callers, ... (wrapping) until `seconds` have passed and
-// every query has been answered at least once.  out_*: the answer recorded for each query index (n_queries x k).
-int hx_callers_run(hx_service* svc, hx_index* index, uint32_t ef, const float* queries, size_t n_queries, uint32_t dim,
-                   uint32_t k, uint32_t n_callers, uint32_t n_threads, int mode, double seconds, uint64_t* out_ids,
-                   float* out_scores, uint32_t* out_counts, hx_callers_report* rep) {
-  if (!queries || !rep || n_callers == 0 || n_queries == 0 || (mode != 2 && !svc) || (mode == 2 && !index)) return 1;
+}
+
+// one blocking call for query qi (service search, or the direct library call), and the async submit for query qi
+using BlockingCall = std::function<void(size_t qi, uint64_t* ids, float* scores, uint32_t* count)>;
+using SubmitCall = std::function<uint64_t(size_t qi)>;
+
+// Caller c walks queries c, c + n_callers, ... (wrapping) until `seconds` have passed and every query has been answered
+// at least once.  out_*: the answer recorded for each query index (n_queries x k).
+static int run_callers(hx_service* svc, size_t n_queries, uint32_t k, uint32_t n_callers, uint32_t n_threads, int mode,
+                       double seconds, const BlockingCall& call, const SubmitCall& submit, uint64_t* out_ids,
+                       float* out_scores, uint32_t* out_counts, hx_callers_report* rep) {
   if (mode != 1) n_threads = n_callers;
   if (n_threads == 0) n_threads = 1;
   n_threads = std::min(n_threads, n_callers);
@@ -49,7 +57,6 @@ int hx_callers_run(hx_service* svc, hx_index* index, uint32_t ef, const float* q
 
   auto worker = [&](uint32_t t) {
     try {
-      helix::SearchService* S = svc ? new helix::SearchService(svc, k, false) : nullptr;
       std::vector<float>& L = lat[t];
       L.reserve(1 << 16);
       while (!go.load(std::memory_order_acquire)) std::this_thread::yield();
@@ -57,18 +64,12 @@ int hx_callers_run(hx_service* svc, hx_index* index, uint32_t ef, const float* q
       if (mode == 0 || mode == 2) {
         std::vector<uint64_t> ids(k);
         std::vector<float> sc(k);
-        hx_search_params p{};
-        p.k = k;
-        p.ef = ef;
-        p.simhash_mode = HX_SIMHASH_OFF;
-        p.pre_sampling_ratio = 1.0f;
         size_t qi = t % n_queries, done_here = 0;
         const size_t mine = (n_queries + n_callers - 1 - t) / n_callers;   // queries this caller must cover once
         while (clk::now() < t_end || done_here < mine) {
           uint32_t cnt = 0;
           const auto a = clk::now();
-          if (mode == 0) S->search(queries + qi * dim, ids.data(), sc.data(), &cnt);
-          else helix::check(hx_search(index, queries + qi * dim, 1, &p, ids.data(), sc.data(), &cnt, nullptr));
+          call(qi, ids.data(), sc.data(), &cnt);
           const auto b = clk::now();
           L.push_back(std::chrono::duration<float, std::micro>(b - a).count());
           record(qi, ids.data(), sc.data(), cnt);
@@ -95,11 +96,13 @@ int hx_callers_run(hx_service* svc, hx_index* index, uint32_t ef, const float* q
               const size_t mine = (n_queries + n_callers - 1 - T.c) / n_callers;
               if (past && T.done >= mine) { finished[i] = true; active--; continue; }
               T.t0 = clk::now();
-              T.ticket = S->submit(queries + T.qi * dim);
+              T.ticket = submit(T.qi);
               T.busy = true;
             } else {
               uint32_t cnt = 0;
-              if (S->poll(T.ticket, ids.data(), sc.data(), &cnt)) {
+              int32_t done = 0;
+              helix::check(hx_service_poll(svc, T.ticket, &done, ids.data(), sc.data(), &cnt));
+              if (done) {
                 L.push_back(std::chrono::duration<float, std::micro>(clk::now() - T.t0).count());
                 record(T.qi, ids.data(), sc.data(), cnt);
                 completed.fetch_add(1, std::memory_order_relaxed);
@@ -112,7 +115,6 @@ int hx_callers_run(hx_service* svc, hx_index* index, uint32_t ef, const float* q
           }
         }
       }
-      delete S;
     } catch (const std::exception&) {
       errors.fetch_add(1);
     }
@@ -142,5 +144,61 @@ int hx_callers_run(hx_service* svc, hx_index* index, uint32_t ef, const float* q
     rep->max_us = all.back();
   }
   return rep->errors ? 2 : 0;
+}
+
+extern "C" {
+// queries: n_queries x dim
+int hx_callers_run(hx_service* svc, hx_index* index, uint32_t ef, const float* queries, size_t n_queries, uint32_t dim,
+                   uint32_t k, uint32_t n_callers, uint32_t n_threads, int mode, double seconds, uint64_t* out_ids,
+                   float* out_scores, uint32_t* out_counts, hx_callers_report* rep) {
+  if (!queries || !rep || n_callers == 0 || n_queries == 0 || (mode != 2 && !svc) || (mode == 2 && !index)) return 1;
+  hx_search_params p{};
+  p.k = k;
+  p.ef = ef;
+  p.simhash_mode = HX_SIMHASH_OFF;
+  p.pre_sampling_ratio = 1.0f;
+  const helix::SearchService S(svc, k, false);
+  const BlockingCall call = [&](size_t qi, uint64_t* ids, float* sc, uint32_t* cnt) {
+    if (mode == 0) S.search(queries + qi * dim, ids, sc, cnt);
+    else helix::check(hx_search(index, queries + qi * dim, 1, &p, ids, sc, cnt, nullptr));
+  };
+  const SubmitCall submit = [&](size_t qi) { return S.submit(queries + qi * dim); };
+  return run_callers(svc, n_queries, k, n_callers, n_threads, mode, seconds, call, submit, out_ids, out_scores, out_counts,
+                     rep);
+}
+
+// search_restricted callers: query qi scans cand_ids[cand_offsets[qi] .. cand_offsets[qi + 1]), or the device set
+// sets[qi] when `sets` is given (the direct mode then calls hx_search_restricted_sets with that one set)
+int hx_callers_run_restricted(hx_service* svc, hx_index* index, const float* queries, size_t n_queries, uint32_t dim,
+                              uint32_t k, const uint64_t* cand_ids, const uint64_t* cand_offsets, hx_candidates* const* sets,
+                              uint32_t n_callers, uint32_t n_threads, int mode, double seconds, uint64_t* out_ids,
+                              float* out_scores, uint32_t* out_counts, hx_callers_report* rep) {
+  if (!queries || !rep || n_callers == 0 || n_queries == 0 || (mode != 2 && !svc) || (mode == 2 && !index) ||
+      (!sets && (!cand_ids || !cand_offsets)))
+    return 1;
+  hx_search_params p{};
+  p.k = k;
+  p.simhash_mode = HX_SIMHASH_OFF;
+  p.pre_sampling_ratio = 1.0f;
+  const helix::RestrictedSearchService S(svc, k, false);
+  const BlockingCall call = [&](size_t qi, uint64_t* ids, float* sc, uint32_t* cnt) {
+    const float* q = queries + qi * dim;
+    if (sets) {
+      if (mode == 0) helix::check(hx_service_search_restricted_set(svc, q, sets[qi], ids, sc, cnt));
+      else helix::check(hx_search_restricted_sets(index, q, 1, &p, sets + qi, 1, ids, sc, cnt, nullptr));
+      return;
+    }
+    const uint64_t* c = cand_ids + cand_offsets[qi];
+    const size_t n = cand_offsets[qi + 1] - cand_offsets[qi];
+    if (mode == 0) S.search(q, c, n, ids, sc, cnt);
+    else helix::check(hx_search_restricted(index, q, 1, &p, c, n, ids, sc, cnt, nullptr));
+  };
+  const SubmitCall submit = [&](size_t qi) {
+    const float* q = queries + qi * dim;
+    if (sets) return S.submit(q, sets[qi]);
+    return S.submit(q, cand_ids + cand_offsets[qi], cand_offsets[qi + 1] - cand_offsets[qi]);
+  };
+  return run_callers(svc, n_queries, k, n_callers, n_threads, mode, seconds, call, submit, out_ids, out_scores, out_counts,
+                     rep);
 }
 }

@@ -258,4 +258,61 @@ class SearchService {
   bool owned_ = true;
 };
 
+// hx_restricted_service_create: search_restricted with the same calling pattern (read_index.rs:92-101) — one query and
+// one candidate set per call, many concurrent tasks — served by shared exact-scan launches.  Answers are bit-identical to
+// VectorIndex::search_restricted.  A device set (hx_candidates*) must outlive the tickets that name it.
+class RestrictedSearchService {
+ public:
+  // borrows an index handle (the owner keeps it alive for the service's lifetime)
+  RestrictedSearchService(hx_index* index, uint32_t k, uint64_t arena_ids = 0, uint32_t capacity = 0, uint32_t max_batch = 0)
+      : k_(k) {
+    hx_service_config c{};
+    c.k = k;
+    c.capacity = capacity;
+    c.max_batch = max_batch;
+    check(hx_restricted_service_create(index, &c, arena_ids, &h_));
+  }
+  explicit RestrictedSearchService(hx_service* adopt_borrowed, uint32_t k, bool) : h_(adopt_borrowed), k_(k), owned_(false) {}
+  ~RestrictedSearchService() { if (owned_) hx_service_destroy(h_); }
+  RestrictedSearchService(const RestrictedSearchService&) = delete;
+  RestrictedSearchService& operator=(const RestrictedSearchService&) = delete;
+
+  uint64_t submit(const float* query, const uint64_t* cand_ids, size_t n_cand) const {
+    uint64_t t = 0;
+    check(hx_service_submit_restricted(h_, query, cand_ids, n_cand, &t));
+    return t;
+  }
+  uint64_t submit(const float* query, const hx_candidates* set) const {
+    uint64_t t = 0;
+    check(hx_service_submit_restricted_set(h_, query, set, &t));
+    return t;
+  }
+  // false while the query is running; true once `out` holds its results (the ticket is consumed)
+  bool poll(uint64_t ticket, uint64_t* ids, float* scores, uint32_t* count) const {
+    int32_t done = 0;
+    check(hx_service_poll(h_, ticket, &done, ids, scores, count));
+    return done != 0;
+  }
+  void search(const float* query, const uint64_t* cand_ids, size_t n_cand, uint64_t* ids, float* scores,
+              uint32_t* count) const {
+    check(hx_service_search_restricted(h_, query, cand_ids, n_cand, ids, scores, count));
+  }
+  std::vector<SearchResult> search(const std::vector<float>& query, const RestrictedVectorCandidates& allowed) const {
+    std::vector<uint64_t> ids(k_);
+    std::vector<float> scores(k_);
+    uint32_t count = 0;
+    search(query.data(), allowed.ids().data(), allowed.ids().size(), ids.data(), scores.data(), &count);
+    std::vector<SearchResult> out(count);
+    for (uint32_t i = 0; i < count; ++i) out[i] = SearchResult{ids[i], scores[i]};
+    return out;
+  }
+  uint32_t k() const { return k_; }
+  hx_service* raw() const { return h_; }
+
+ private:
+  hx_service* h_ = nullptr;
+  uint32_t k_;
+  bool owned_ = true;
+};
+
 }   // namespace helix

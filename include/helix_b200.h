@@ -400,6 +400,38 @@ hx_status hx_service_search(hx_service* svc, const float* query, uint64_t* out_i
                             uint32_t* out_count);
 hx_status hx_service_get_stats(hx_service* svc, hx_service_stats* out);
 
+/* ---- restricted query service: search_restricted with the same calling pattern ---------------------------------
+ * ValidatedVectorReadIndex::search_restricted (read_index.rs:92-101) is called like search: one (query, candidate set)
+ * per call from many concurrent tasks.  A restricted service coalesces those callers exactly as above, through the same
+ * ring, dispatcher, completer, poll / wait and stats; each coalesced run becomes ONE exact-scan launch that writes every
+ * answer into its host-mapped result slot.  Answers are bit-identical to hx_search_restricted (ids, order, score bits,
+ * count).  No graph or entry point is needed.
+ * Config: k in 1..800 (restricted.rs:55); capacity, max_batch (<= 128), n_streams, min_batch, batch_window_us and flags
+ * as above (HX_SERVICE_STAGE_QUERIES stages candidate ids too); ef, ctas_per_sm, cta_warps, rows_in_flight and
+ * visited_log2 must be 0.  arena_ids sizes the pinned arena that holds submitted candidate ids until their launch has
+ * read them: 0 => 2000000, values below 1000000 are refused (every legal set fits).  A full arena is back-pressure.
+ * Device memory per service, per stream (n_streams, default 32): (arena_ids / 256 + 128) * 256 B of partial lists, and for
+ * k > 32 (arena_ids + 262144) * 8 B of scores — with the defaults about 65 MB, plus about 580 MB when k > 32.  Fewer
+ * streams (or a smaller arena) cost proportionally less.
+ * hx_service_submit on a restricted service, and the restricted submits on an HNSW service, are HX_ERR_INVALID_PARAMETER. */
+hx_status hx_restricted_service_create(hx_index* idx, const hx_service_config* cfg, uint64_t arena_ids, hx_service** out);
+/* Admission on the caller's thread, in restricted_host's order: |C| > 1e6 => HX_ERR_QUERY; an empty set completes the
+ * ticket at once with count 0 (no query validation, no device work); ids not ascending and unique =>
+ * HX_ERR_INVALID_PARAMETER; then the query is validated (dimension -> finiteness -> cosine zero norm -> magnitude).
+ * The ids are copied: the caller's array may be reused when the call returns. */
+hx_status hx_service_submit_restricted(hx_service* svc, const float* query, const uint64_t* cand_ids, size_t n_cand,
+                                       uint64_t* out_ticket);
+/* Same with a device-resident set (hx_candidates_create): no ids cross PCIe.  A set of another index or of an older
+ * vector generation is HX_ERR_INVARIANT_VIOLATION.  The set is read by the device until the ticket completes: it must
+ * not be destroyed before hx_service_poll / hx_service_wait has returned the ticket's results. */
+hx_status hx_service_submit_restricted_set(hx_service* svc, const float* query, const hx_candidates* set,
+                                           uint64_t* out_ticket);
+/* submit + wait: the drop-in for one ValidatedVectorReadIndex::search_restricted call. */
+hx_status hx_service_search_restricted(hx_service* svc, const float* query, const uint64_t* cand_ids, size_t n_cand,
+                                       uint64_t* out_ids, float* out_scores, uint32_t* out_count);
+hx_status hx_service_search_restricted_set(hx_service* svc, const float* query, const hx_candidates* set,
+                                           uint64_t* out_ids, float* out_scores, uint32_t* out_count);
+
 /* ---- search (device buffers: inputs already resident in HBM) ------------------------- */
 /* Same semantics, no validation copy, no host sync: everything is enqueued on
  * `cuda_stream` (a cudaStream_t, 0 = legacy default stream).  d_queries must have been
