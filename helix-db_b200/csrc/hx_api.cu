@@ -169,7 +169,9 @@ void hx_index::free_vectors() {
   if (d_simhash) cudaFree(d_simhash);
   if (d_has_simhash) cudaFree(d_has_simhash);
   d_simhash = nullptr; d_has_simhash = nullptr; simhash_count = 0;
-  d_vec = nullptr; d_hdr = nullptr; d_ids = nullptr; d_vec_bf16 = nullptr; d_sqnorm = nullptr;
+  if (d_live_slots) cudaFree(d_live_slots);
+  d_vec = nullptr; d_hdr = nullptr; d_ids = nullptr; d_vec_bf16 = nullptr; d_sqnorm = nullptr; d_live_slots = nullptr;
+  n_live = 0;
   if (d_deleted) cudaFree(d_deleted);
   d_deleted = nullptr;
   host_deleted.clear();

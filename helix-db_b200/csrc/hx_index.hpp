@@ -184,7 +184,11 @@ struct hx_index {
   uint8_t* d_has_simhash = nullptr;    // [n]
   float* d_planes_t = nullptr;         // [dim][64] (transposed for coalesced projection)
   size_t simhash_count = 0;
-  // bf16 copy for the dense path
+  // dense path state (k_dense.cu), built on first use after every mirror write and published under dense_mu only once
+  // complete: the ascending slots of the live (not deleted) rows, and the bf16 copy of those rows compacted in that order
+  std::mutex dense_mu;
+  uint32_t* d_live_slots = nullptr;
+  size_t n_live = 0;
   void* d_vec_bf16 = nullptr;
   float* d_sqnorm = nullptr;
   // scratch pool

@@ -13,7 +13,7 @@
 //   * fused epilogue: the accumulators of each 128 x 128 half tile are written to shared memory (row stride 129 floats, so
 //     the column-order reads below are free of bank conflicts); each of the 256 consumer threads — one query row x one
 //     64-column quarter — turns them into the metric's score order with the stored row norms and keeps the HXD_T best rows
-//     per (query, run of tiles, column quarter) by register insertion, emitting score_bits<<32|slot keys — the B x N
+//     per (query, run of tiles, column quarter) by register insertion, emitting score_bits<<32|row keys — the B x N
 //     score matrix is never written.  Per half tile the epilogue is 64 columns per thread against the 4 x ldb/64 wgmma
 //     steps of the contraction, so it runs between the MMAs of consecutive half tiles instead of beside them.
 // The approximate (bf16) keys only NOMINATE candidates: k_select keeps the k' best keys per query and the exact fp32
@@ -120,7 +120,7 @@ __device__ __forceinline__ uint64_t hxd_make_desc(uint32_t smem_addr) {
 }
 
 struct HxDenseArgs {
-  uint32_t n_rows;            // corpus rows (unpadded)
+  uint32_t n_rows;            // rows of the bf16 copy = live corpus rows (unpadded)
   uint32_t n_queries;         // B (unpadded)
   uint32_t k_blocks;          // ldb / 64
   uint32_t m_tiles, n_tiles;  // 128-query tiles, 256-row corpus tiles
@@ -296,13 +296,14 @@ k_dense_scores(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
 // f32 rows -> bf16 rows (round to nearest even) with zero padding to ldb, plus the per-row aux term computed from the
 // ROUNDED values (so that approximate scores are self-consistent)
 // `tiled`: the corpus copy — row w goes to its tile position (hxd_pos_of_row); queries keep their order
+// `src_rows`: row w of the copy is source row src_rows[w] (the live slots: deleted rows are left out); nullptr = row w
 __global__ void k_to_bf16(const float* __restrict__ src, size_t rows, uint32_t dim, size_t ld_src, __nv_bfloat16* __restrict__ dst,
-                          uint32_t ldb, float* __restrict__ aux, int metric, int tiled) {
+                          uint32_t ldb, float* __restrict__ aux, int metric, int tiled, const uint32_t* __restrict__ src_rows) {
   const size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint32_t lane = threadIdx.x & 31u;
   if (w >= rows) return;
   const size_t pos = tiled ? (w / HXD_BN) * HXD_BN + hxd_pos_of_row((uint32_t)(w % HXD_BN)) : w;
-  const float* s = src + w * ld_src;
+  const float* s = src + (src_rows ? (size_t)src_rows[w] : w) * ld_src;
   __nv_bfloat16* d = dst + pos * (size_t)ldb;
   float ss = 0.f;
   for (uint32_t j = lane; j < ldb; j += 32) {
@@ -318,10 +319,39 @@ __global__ void k_to_bf16(const float* __restrict__ src, size_t rows, uint32_t d
   if (lane == 0) aux[pos] = metric == HXM_COSINE ? (ss > 0.f ? rsqrtf(ss) : 0.f) : ss;
 }
 
-// keys[q][j] hold GLOBAL slots in their low word; turn the selected ones into a per-query candidate slot list
-__global__ void k_keys_to_slots(const uint64_t* __restrict__ sel_ids_as_slots, size_t total, uint32_t* __restrict__ out) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < total) out[i] = (uint32_t)sel_ids_as_slots[i];
+// The k' nominees of a query (rows of the bf16 copy in the low word, in approximate-score order; HX_ABSENT = unfilled) ->
+// its candidate slot list for the exact re-rank, ASCENDING.  k_scan keys a candidate by its position in this list, so
+// ascending slots make exact ties resolve by id — the reference's (score, id) rule — in order and in which tied rows
+// make the cut, instead of by their bf16 scores.  One CTA per query sorts `width` (a power of two >= k') entries.
+#define HXD_SORT_THREADS 256
+#define HXD_SORT_MAX 1024
+__global__ void __launch_bounds__(HXD_SORT_THREADS) k_nominee_slots(const uint64_t* __restrict__ sel, size_t B, uint32_t kprime,
+                                                                   uint32_t width, const uint32_t* __restrict__ live_slots,
+                                                                   uint32_t* __restrict__ out) {
+  __shared__ uint32_t s[HXD_SORT_MAX];
+  for (size_t q = blockIdx.x; q < B; q += gridDim.x) {
+    for (uint32_t i = threadIdx.x; i < width; i += HXD_SORT_THREADS) {
+      uint32_t v = HX_ABSENT;
+      if (i < kprime) {
+        const uint32_t w = (uint32_t)sel[q * kprime + i];
+        if (w != HX_ABSENT) v = live_slots[w];
+      }
+      s[i] = v;
+    }
+    for (uint32_t size = 2; size <= width; size <<= 1)
+      for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+        __syncthreads();
+        for (uint32_t p = threadIdx.x; p < width / 2; p += HXD_SORT_THREADS) {
+          const uint32_t i = 2 * p - (p & (stride - 1)), j = i + stride;
+          const bool up = (i & size) == 0;
+          const uint32_t x = s[i], y = s[j];
+          if ((x > y) == up) { s[i] = y; s[j] = x; }
+        }
+      }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < kprime; i += HXD_SORT_THREADS) out[q * kprime + i] = s[i];
+    __syncthreads();
+  }
 }
 
 // ---- host ------------------------------------------------------------------------------------------------------------------
@@ -353,17 +383,52 @@ static hx_status make_map(CUtensorMap* map, void* base, uint64_t rows, uint32_t 
   return HX_OK;
 }
 
-// lazily build the bf16 copy of the corpus
-static hx_status ensure_bf16(hx_index* ix, uint32_t ldb) {
-  if (ix->d_vec_bf16) return HX_OK;
-  const size_t n_pad = (ix->n + HXD_BN - 1) / HXD_BN * HXD_BN;
-  HX_CUDA(cudaMalloc(&ix->d_vec_bf16, n_pad * (size_t)ldb * 2));
-  HX_CUDA(cudaMemset(ix->d_vec_bf16, 0, n_pad * (size_t)ldb * 2));
-  HX_CUDA(cudaMalloc((void**)&ix->d_sqnorm, n_pad * sizeof(float)));
-  HX_CUDA(cudaMemset(ix->d_sqnorm, 0, n_pad * sizeof(float)));
-  k_to_bf16<<<(unsigned)((ix->n + 7) / 8), 256>>>(ix->d_vec, ix->n, ix->cfg.dimension, ix->ld, (__nv_bfloat16*)ix->d_vec_bf16, ldb,
-                                                  ix->d_sqnorm, ix->cfg.metric, 1);
-  HX_CUDA(cudaGetLastError());
+// Lazily build the dense path's view of the corpus (dropped by every mirror write, hx_mirror.inl: invalidate_bf16): the
+// ascending live slots and, when `need_bf16`, the bf16 copy of the live rows compacted in slot order (deleted rows take
+// no tile column and no bucket space).  The work is enqueued on the calling stream and the pointers are published under
+// ix->dense_mu only after that stream has completed it, so a caller on any other stream never reads a half-built copy,
+// and concurrent first callers build it once.
+static hx_status ensure_dense_state(hx_index* ix, uint32_t ldb, bool need_bf16, cudaStream_t stream) {
+  std::lock_guard<std::mutex> lk(ix->dense_mu);
+  if (!ix->d_live_slots) {
+    std::vector<uint32_t> live;
+    live.reserve(ix->n - std::min(ix->n, ix->n_deleted));
+    for (size_t s = 0; s < ix->n; ++s)
+      if (ix->host_deleted.empty() || !ix->host_deleted[s]) live.push_back((uint32_t)s);
+    uint32_t* d = nullptr;
+    HX_CUDA(cudaMalloc((void**)&d, std::max<size_t>(live.size(), 1) * sizeof(uint32_t)));
+    cudaError_t e = cudaMemcpyAsync(d, live.data(), live.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) {
+      cudaFree(d);
+      hx_set_error("dense path live-row table: %s", cudaGetErrorString(e));
+      return HX_ERR_CUDA;
+    }
+    ix->d_live_slots = d;
+    ix->n_live = live.size();
+  }
+  if (!need_bf16 || ix->d_vec_bf16) return HX_OK;
+  const size_t n = ix->n_live, n_pad = (n + HXD_BN - 1) / HXD_BN * HXD_BN;
+  void* vb = nullptr;
+  float* aux = nullptr;
+  cudaError_t e = cudaMalloc(&vb, n_pad * (size_t)ldb * 2);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&aux, n_pad * sizeof(float));
+  if (e == cudaSuccess) e = cudaMemsetAsync(vb, 0, n_pad * (size_t)ldb * 2, stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(aux, 0, n_pad * sizeof(float), stream);
+  if (e == cudaSuccess) {
+    k_to_bf16<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(ix->d_vec, n, ix->cfg.dimension, ix->ld, (__nv_bfloat16*)vb, ldb, aux,
+                                                          ix->cfg.metric, 1, ix->d_live_slots);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+  if (e != cudaSuccess) {
+    if (vb) cudaFree(vb);
+    if (aux) cudaFree(aux);
+    hx_set_error("dense path bf16 copy: %s", cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? HX_ERR_OUT_OF_MEMORY : HX_ERR_CUDA;
+  }
+  ix->d_vec_bf16 = vb;
+  ix->d_sqnorm = aux;
   return HX_OK;
 }
 
@@ -397,6 +462,75 @@ static hx_status dense_check(hx_index* ix, const hx_search_params* p) {
   return HX_OK;
 }
 
+// validation + exact headers (same order of checks as every other entry point)
+static void dense_validate(hx_index* ix, const float* d_q, size_t B, float* d_qhdr, uint32_t* d_status, cudaStream_t stream) {
+  const uint32_t dim = ix->cfg.dimension;
+  float limit = 0.f;
+  bool has_limit = false;
+  if (ix->cfg.metric == HX_METRIC_EUCLIDEAN) {
+    const double exact = std::sqrt((double)FLT_MAX / ((double)dim * 8.0));
+    limit = (float)exact;
+    if ((double)limit > exact) limit = std::nextafter(limit, 0.0f);
+    has_limit = true;
+  }
+  k_validate_and_header<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(d_q, B, dim, dim, ix->cfg.metric, limit, has_limit ? 1 : 0,
+                                                                    d_qhdr, d_status);
+}
+
+// Small corpora (see hx_dense_device): every query scans every live row with the exact kernel, keyed by position in the
+// ascending live-slot table, and keeps the k smallest (score, id) — the answer of restricted_exact_scan over all ids.
+static hx_status dense_exact_scan(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
+                                  uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
+                                  cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out) {
+  const size_t n = ix->n_live;
+  if (n == 0) {
+    HX_CUDA(cudaMemsetAsync(d_out_cnt, 0, B * sizeof(uint32_t), stream));
+    if (launches_out) *launches_out = 0;
+    return HX_OK;
+  }
+  hx_status rc;
+  DevBuf<uint8_t>& kb = scr->misc[15];   // not one of the tensor-core pass's buffers: its cached tensor maps stay valid
+  if ((rc = kb.reserve(B * n * 8)) || (rc = scr->d_qhdr.reserve(B)) || (rc = scr->d_qstatus.reserve(B)) ||
+      (rc = scr->d_err.reserve(4)))
+    return rc;
+  uint64_t* d_keys = reinterpret_cast<uint64_t*>(kb.p);
+  HX_CUDA(cudaMemsetAsync(scr->d_err.p, 0, 4, stream));
+  dense_validate(ix, d_q, B, scr->d_qhdr.p, scr->d_qstatus.p, stream);
+  HxDev dev = ix->dev();
+  HxScanArgs sa{};
+  sa.queries = d_q;
+  sa.q_hdr = scr->d_qhdr.p;
+  sa.q_status = scr->d_qstatus.p;
+  sa.B = (uint32_t)B;
+  sa.cand_slots = ix->d_live_slots;
+  sa.keys = d_keys;
+  sa.shared_set = 1;
+  sa.n_shared = n;
+  sa.chunk = 1024;
+  sa.err_flags = scr->d_err.p;
+  dim3 g((unsigned)((n + sa.chunk - 1) / sa.chunk), (unsigned)std::min<size_t>(B, 65535));
+  const uint32_t sm = ix->ld * 4u;
+  if (e0) HX_CUDA(cudaEventRecord(e0, stream));
+  if (ix->cfg.metric == HX_METRIC_COSINE) k_scan<HXM_COSINE><<<g, HX_SCAN_THREADS, sm, stream>>>(dev, sa);
+  else k_scan<HXM_EUCLIDEAN><<<g, HX_SCAN_THREADS, sm, stream>>>(dev, sa);
+  if (e1) HX_CUDA(cudaEventRecord(e1, stream));
+  HxSelectArgs s2{};
+  s2.keys = d_keys;
+  s2.cand_slots = ix->d_live_slots;
+  s2.q_status = scr->d_qstatus.p;
+  s2.B = (uint32_t)B;
+  s2.k = p->k;
+  s2.shared_set = 1;
+  s2.n_shared = n;
+  s2.out_ids = d_out_ids;
+  s2.out_scores = d_out_sc;
+  s2.out_counts = d_out_cnt;
+  k_select<<<(unsigned)std::min<size_t>(B, 65535), HX_SEL_THREADS, 0, stream>>>(dev, s2);
+  HX_CUDA(cudaGetLastError());
+  if (launches_out) *launches_out = 3;
+  return HX_OK;
+}
+
 // Everything below is enqueued on `stream`; nothing synchronises with the host (buffers, tensor maps and the nominee
 // offsets are cached in the scratch set across calls).  d_queries: B x dim f32 on the device.  Per-query validation status
 // is left in s->d_qstatus (a query that fails validation yields count 0); error flags accumulate in s->d_err[0].
@@ -412,12 +546,20 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
   }
   const uint32_t dim = ix->cfg.dimension, k = p->k;
   const uint32_t ldb = (dim + HXD_BK - 1) / HXD_BK * HXD_BK;
-  if ((rc = ensure_bf16(ix, ldb))) return rc;
-  const size_t n = ix->n;
+  if ((rc = ensure_dense_state(ix, ldb, false, stream))) return rc;
+  const size_t n = ix->n_live;   // rows of the bf16 copy: the live rows, compacted
+  // Small corpora get the exact scan over every live row.  The tensor-core pass hands each query at most
+  // HXD_PARTS * HXD_T = 32 nominees per run of tiles, and a run is at least one 256-row tile, so a corpus of few tiles
+  // cannot fill k' = min(max(4k, 64), 800, live rows) nominees, and its count could fall short of min(k, live rows).
+  // From 8 * min(max(4k, 64), 800) live rows on, every run but the last holds a full tile (32 nominees), which covers k'
+  // (n_split below is at least k'/4 runs or every tile).  Below that the exact scan costs at most 6400 rows per query.
+  const uint32_t kcap = std::min<uint32_t>(std::max<uint32_t>(4 * k, 64), 800);
+  if (n < 8 * (size_t)kcap) return dense_exact_scan(ix, scr, d_q, B, p, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out);
+  if ((rc = ensure_dense_state(ix, ldb, true, stream))) return rc;
   const uint32_t m_tiles = (uint32_t)((B + HXD_BM - 1) / HXD_BM), n_tiles = (uint32_t)((n + HXD_BN - 1) / HXD_BN);
   const size_t B_pad = (size_t)m_tiles * HXD_BM, n_pad = (size_t)n_tiles * HXD_BN;
   const size_t n_ctas = (size_t)std::max(1, ix->sm_count);   // one persistent CTA per SM
-  const uint32_t kprime = (uint32_t)std::min<size_t>(std::max<uint32_t>(4 * k, 64), std::min<size_t>(800, n));
+  const uint32_t kprime = (uint32_t)std::min<size_t>(kcap, n);
   // runs per query tile: enough units to fill the CTAs, and enough that one run's best-T comfortably covers its share
   // of the k' nominees even when the true neighbours cluster in id space (8x head-room)
   uint32_t n_split = (uint32_t)std::max<size_t>(1, std::min<size_t>(n_tiles,
@@ -471,18 +613,8 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
     dc.map_x_rows = n_pad;
   }
   uint32_t launches = 0;
-  // validation + exact headers (same order of checks as every other entry point)
-  float limit = 0.f;
-  bool has_limit = false;
-  if (ix->cfg.metric == HX_METRIC_EUCLIDEAN) {
-    const double exact = std::sqrt((double)FLT_MAX / ((double)dim * 8.0));
-    limit = (float)exact;
-    if ((double)limit > exact) limit = std::nextafter(limit, 0.0f);
-    has_limit = true;
-  }
-  k_validate_and_header<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(d_q, B, dim, dim, ix->cfg.metric, limit, has_limit ? 1 : 0,
-                                                                    d_qhdr, d_status);
-  k_to_bf16<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(d_q, B, dim, dim, d_qb, ldb, d_qaux, ix->cfg.metric, 0);
+  dense_validate(ix, d_q, B, d_qhdr, d_status, stream);
+  k_to_bf16<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(d_q, B, dim, dim, d_qb, ldb, d_qaux, ix->cfg.metric, 0, nullptr);
   launches += 2;
   HX_CUDA(cudaGetLastError());
   // ---- tensor-core pass ----
@@ -517,13 +649,16 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
   s1.q_status = d_status;
   s1.B = (uint32_t)B;
   s1.k = kprime;
-  s1.shared_set = 2;   // keys carry global slots in their low word (no candidate indirection)
+  s1.shared_set = 2;   // keys carry rows of the bf16 copy in their low word (no candidate indirection)
   s1.n_shared = (uint64_t)n_split * HXD_PARTS * HXD_T;
   s1.out_ids = d_sel_ids;
   s1.out_scores = d_sel_sc;
   s1.out_counts = d_sel_cnt;
   k_select<<<(unsigned)std::min<size_t>(B, 65535), HX_SEL_THREADS, 0, stream>>>(dev, s1);
-  k_keys_to_slots<<<(unsigned)((B * (size_t)kprime + 255) / 256), 256, 0, stream>>>(d_sel_ids, B * (size_t)kprime, d_cslots);
+  uint32_t width = 32;
+  while (width < kprime) width <<= 1;
+  k_nominee_slots<<<(unsigned)std::min<size_t>(B, 65535), HXD_SORT_THREADS, 0, stream>>>(d_sel_ids, B, kprime, width,
+                                                                                       ix->d_live_slots, d_cslots);
   launches += 2;
   HxScanArgs sa{};
   sa.queries = d_q;

@@ -11,6 +11,7 @@ import pytest
 import helix_db_b200 as hx
 from helix_db_b200 import sharding as sh
 from oracle import hxo
+from hx_testutil import mirror_from_oracle
 from test_gpu_parity import build_pair
 
 pytestmark = pytest.mark.gpu
@@ -38,6 +39,20 @@ def test_group_of_one_matches_unsharded():
         assert rids[b, :rcnt[b]].tolist() == ei.tolist() and rsc[b, :rcnt[b]].tobytes() == es.tobytes()
     local_ms, coll_ms = g.last_ms()
     assert local_ms > 0.0
+    # the dense path (needs the bf16 copy: storage = 1): a group of one gives the unsharded hx_search_dense answer
+    gpu_d = hx.VectorIndex(hx.Metric.Cosine, hx.VectorIndexConfig("t", "embedding", dim), storage=1)
+    mirror_from_oracle(gpu_d, ora)
+    g_d = sh.ShardGroup(gpu_d, 1, 0, None)
+    di, ds, dc = g_d.search(sh.DENSE, q, hx.SearchParams.strict(k), k)
+    ui, us, uc = gpu_d.search_dense_batch(q, hx.SearchParams.strict(k))
+    assert dc.tolist() == uc.tolist() == [k] * B
+    assert di.tolist() == ui.tolist() and ds.tobytes() == us.tobytes()
+    for b in range(0, B, 10):
+        ei, es = ora.search_exact(q[b], k)
+        exact = dict(zip(ei.tolist(), es.view(np.uint32).tolist()))
+        assert all(exact[i] == s for i, s in zip(di[b].tolist(), ds[b].view(np.uint32).tolist()) if i in exact)
+    g_d.close()
+    gpu_d.close()
     g.close()
     gpu.close()
 
