@@ -297,6 +297,10 @@ k_dense_scores(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
 // ROUNDED values (so that approximate scores are self-consistent)
 // `tiled`: the corpus copy — row w goes to its tile position (hxd_pos_of_row); queries keep their order
 // `src_rows`: row w of the copy is source row src_rows[w] (the live slots: deleted rows are left out); nullptr = row w
+// Cosine is scale-free, and cosine vectors have no component limit: before rounding, each row / query is multiplied by the
+// power of two that brings its largest |component| into [1, 2) (exact).  Without it a norm of ~1e19 or more makes the fp32
+// sum of squares inf, one of ~1e-29 or less makes it 0 (the row term 0: every approximate score 0.5), and FLT_MAX rounds to
+// a bf16 inf.  Euclidean rows keep their scale: the score is not scale-free, and every legal row fits (component limit).
 __global__ void k_to_bf16(const float* __restrict__ src, size_t rows, uint32_t dim, size_t ld_src, __nv_bfloat16* __restrict__ dst,
                           uint32_t ldb, float* __restrict__ aux, int metric, int tiled, const uint32_t* __restrict__ src_rows) {
   const size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -305,9 +309,22 @@ __global__ void k_to_bf16(const float* __restrict__ src, size_t rows, uint32_t d
   const size_t pos = tiled ? (w / HXD_BN) * HXD_BN + hxd_pos_of_row((uint32_t)(w % HXD_BN)) : w;
   const float* s = src + (src_rows ? (size_t)src_rows[w] : w) * ld_src;
   __nv_bfloat16* d = dst + pos * (size_t)ldb;
+  int shift = 0;
+  if (metric == HXM_COSINE) {
+    float mx = 0.f;
+    for (uint32_t j = lane; j < dim; j += 32) mx = fmaxf(mx, fabsf(s[j]));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 16)); mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 8));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 4));  mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    if (mx > 0.f) {
+      int e;
+      frexpf(mx, &e);   // mx = m * 2^e, m in [0.5, 1): mx * 2^(1-e) is in [1, 2)
+      shift = 1 - e;
+    }
+  }
   float ss = 0.f;
   for (uint32_t j = lane; j < ldb; j += 32) {
-    const float x = j < dim ? s[j] : 0.f;
+    const float x = j < dim ? ldexpf(s[j], shift) : 0.f;
     const __nv_bfloat16 b = __float2bfloat16_rn(x);
     d[j] = b;
     const float xb = __bfloat162float(b);

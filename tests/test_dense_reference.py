@@ -27,12 +27,25 @@ def bf16_round(x):
     return r.view(np.float32).reshape(a.shape)
 
 
+def pow2_normalize(a):
+    """Each row times the power of two that brings its largest |component| into [1, 2) (k_to_bf16 does this for cosine
+    before rounding); all-zero rows are left alone.  One rounding at most (a result below 2^-126), as ldexpf."""
+    a = np.asarray(a, dtype=np.float32)
+    m = np.abs(a).max(axis=1)
+    _, e = np.frexp(m)
+    shift = np.where(m > 0, 1 - e, 0)
+    return np.ldexp(a.astype(np.float64), shift[:, None]).astype(np.float32)
+
+
 def emulate(metric, queries, rows):
     """Approximate scores of k_dense_scores in float64, [B, n], and the per-(query, row) epsilon bounding its fp32 error.
 
     cosine:    0.5 - 0.5 <q^, x^> / (|q^| |x^|)            euclidean: |q^|^2 + |x^|^2 - 2 <q^, x^>        (both clamped at 0)
     epsilon:   2^-14 (cosine)                              2^-14 (sum_j |q^_j x^_j| + |q^|^2 + |x^|^2)
+    q^, x^ are the bf16-rounded operands; for cosine, of the rows after pow2_normalize, as in k_to_bf16.
     """
+    if metric == hxo.COSINE:
+        queries, rows = pow2_normalize(queries), pow2_normalize(rows)
     q = bf16_round(queries).astype(np.float64)
     x = bf16_round(rows).astype(np.float64)
     dot = q @ x.T
@@ -150,3 +163,59 @@ def test_tie_fixture_is_an_exact_tie_in_reversed_bf16_order():
     # ... and far rows never come near
     far, _ = emulate(hxo.EUCLIDEAN, q[None, :], np.delete(rows, pos, axis=0))
     assert far.min() > 100.0
+
+
+# ---- the emulation over the full float32 range (tests/numeric_range.py) -------------------------------------------------------
+def test_emulate_is_finite_over_the_float32_range():
+    import numeric_range as nr
+    for metric in (hxo.COSINE, hxo.EUCLIDEAN):
+        for d in nr.DIMS:
+            ids, rows, queries = nr.corpus(metric, d)
+            approx, eps = emulate(metric, queries, rows)
+            assert np.isfinite(approx).all() and np.isfinite(eps).all(), (metric, d)
+            assert (approx >= 0).all() and (eps >= 0).all()
+    # FLT_MAX rows and the 2^-149 row score like any other direction: a row against itself is 0, its negation 1
+    f = np.float32(np.finfo(np.float32).max)
+    x = np.array([[f, -f, f], [0.0, 2.0 ** -149, 0.0], [3e-39, 1e-45, 0.0]], np.float32)
+    a, _ = emulate(hxo.COSINE, np.concatenate([x, -x]), x)
+    assert np.allclose(np.diag(a[:3]), 0.0, atol=1e-6) and np.allclose(np.diag(a[3:]), 1.0, atol=1e-6)
+
+
+def test_pow2_normalize_is_exact_and_lands_in_one_to_two():
+    rng = np.random.default_rng(9)
+    x = (rng.standard_normal((50, 33)) * np.exp2(rng.integers(-100, 100, 50))[:, None]).astype(np.float32)
+    y = pow2_normalize(x)
+    m = np.abs(y).max(1)
+    assert ((m >= 1.0) & (m < 2.0)).all()
+    assert (np.abs(pow2_normalize(x * np.float32(2.0 ** -20)) - y) == 0).all()
+    f = np.float32(np.finfo(np.float32).max)
+    assert pow2_normalize(np.array([[f, 0.0]], np.float32)).tolist() == [[float(np.nextafter(np.float32(2), np.float32(0))), 0.0]]
+    assert pow2_normalize(np.array([[2.0 ** -149, 0.0]], np.float32)).tolist() == [[1.0, 0.0]]
+
+
+@pytest.mark.parametrize("e", [-100, -70, -1, 1, 60, 100])
+def test_cosine_emulation_is_unchanged_by_a_power_of_two(e):
+    """Scaling one row, or one query, by 2^e leaves every cosine score and epsilon as they were (the scaled values are
+    exact in float32 here: normal, below FLT_MAX)."""
+    rng = np.random.default_rng(e + 500)
+    q = rng.standard_normal((6, 70)).astype(np.float32)
+    x = rng.standard_normal((40, 70)).astype(np.float32)
+    a0, e0 = emulate(hxo.COSINE, q, x)
+    s = np.float32(2.0 ** e)
+    x2, q2 = x.copy(), q.copy()
+    x2[7] *= s
+    q2[2] *= s
+    assert (x2[7].astype(np.float64) == x[7].astype(np.float64) * 2.0 ** e).all()
+    a1, e1 = emulate(hxo.COSINE, q2, x2)
+    assert a1.tobytes() == a0.tobytes() and e1.tobytes() == e0.tobytes()
+
+
+@pytest.mark.parametrize("e", [-60, -20, 20, 40])
+def test_euclidean_emulation_scales_by_four_to_the_e(e):
+    rng = np.random.default_rng(e + 900)
+    q = rng.standard_normal((6, 70)).astype(np.float32)
+    x = rng.standard_normal((40, 70)).astype(np.float32)
+    a0, e0 = emulate(hxo.EUCLIDEAN, q, x)
+    s = np.float32(2.0 ** e)
+    a1, e1 = emulate(hxo.EUCLIDEAN, q * s, x * s)
+    assert (a1 == a0 * 2.0 ** (2 * e)).all() and (e1 == e0 * 2.0 ** (2 * e)).all()
