@@ -189,6 +189,7 @@ ABI_SYMBOLS = [
     "hx_index_upsert_vectors", "hx_index_set_levels", "hx_index_upsert_neighbor_rows", "hx_index_delete_vectors",
     "hx_index_load_upper_vector_rows", "hx_index_set_version", "hx_index_get_version", "hx_index_build_ex",
     "hx_filtered_budgets", "hx_search_filtered_graph", "hx_index_get_tuning", "hx_index_set_tuning",
+    "hx_search_dense_restricted", "hx_search_dense_restricted_set",
 ]
 
 _lib = None
@@ -252,6 +253,11 @@ def load_library():
     L.hx_merge_topk_device.argtypes = [C.c_int32, vp, vp, vp, C.c_uint32, sz, C.c_uint32, vp, vp, vp, vp]
     L.hx_search_dense.restype = C.c_int32
     L.hx_search_dense.argtypes = [vp, fp, sz, C.POINTER(_Params), u64p, fp, u32p, C.POINTER(SearchStats)]
+    L.hx_search_dense_restricted.restype = C.c_int32
+    L.hx_search_dense_restricted.argtypes = [vp, fp, sz, C.POINTER(_Params), u64p, sz, u64p, fp, u32p,
+                                             C.POINTER(SearchStats)]
+    L.hx_search_dense_restricted_set.restype = C.c_int32
+    L.hx_search_dense_restricted_set.argtypes = [vp, fp, sz, C.POINTER(_Params), vp, u64p, fp, u32p, C.POINTER(SearchStats)]
     L.hx_last_error.restype = C.c_char_p
     L.hx_last_error_index.restype = C.c_uint32
     L.hx_version.restype = C.c_char_p
@@ -964,6 +970,39 @@ class VectorIndex:
         _ck(self.L.hx_search_dense(self.h, qp, B, C.byref(cp), ids.ctypes.data_as(C.POINTER(C.c_uint64)),
                                    sc.ctypes.data_as(C.POINTER(C.c_float)), cnt.ctypes.data_as(C.POINTER(C.c_uint32)),
                                    C.byref(st)))
+        return ids, sc, cnt
+
+    def search_dense_restricted_batch(self, queries, params: SearchParams, allowed: RestrictedVectorCandidates, stats=None):
+        """hx_search_dense_restricted: the tensor-core path over one candidate set shared by every query."""
+        qa, qp = _f32(queries)
+        B = qa.size // (params.query_dimension or self.dim)
+        cp = params._c()
+        k = cp.k
+        ca, cpnt = _u64(allowed.ids)
+        ids = np.zeros((B, k), dtype=np.uint64)
+        sc = np.zeros((B, k), dtype=np.float32)
+        cnt = np.zeros(B, dtype=np.uint32)
+        st = stats if stats is not None else SearchStats()
+        _ck(self.L.hx_search_dense_restricted(self.h, qp, B, C.byref(cp), cpnt, ca.size,
+                                              ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                              sc.ctypes.data_as(C.POINTER(C.c_float)),
+                                              cnt.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(st)))
+        return ids, sc, cnt
+
+    def search_dense_restricted_sets(self, queries, params: SearchParams, device_set: "DeviceCandidates", stats=None):
+        """hx_search_dense_restricted_set: the same with a device-resident set (cache_candidates)."""
+        qa, qp = _f32(queries)
+        B = qa.size // self.dim
+        cp = params._c()
+        k = cp.k
+        ids = np.zeros((B, k), dtype=np.uint64)
+        sc = np.zeros((B, k), dtype=np.float32)
+        cnt = np.zeros(B, dtype=np.uint32)
+        st = stats if stats is not None else SearchStats()
+        _ck(self.L.hx_search_dense_restricted_set(self.h, qp, B, C.byref(cp), device_set.h,
+                                                  ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                  sc.ctypes.data_as(C.POINTER(C.c_float)),
+                                                  cnt.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(st)))
         return ids, sc, cnt
 
     # ---- device-buffer path (raw pointers, e.g. torch tensors' data_ptr()) ----

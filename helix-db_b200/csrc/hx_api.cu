@@ -2289,6 +2289,128 @@ extern "C" hx_status hx_search_dense(hx_index* ix, const float* queries, size_t 
   return hx_dense_impl(ix, queries, B, p, out_ids, out_scores, out_counts, stats);
 }
 
+// The dense path over one candidate set shared by the B queries: host ids (`cand_ids`, n_cand) or a device set (`set`).
+// Admission is restricted_host's, in its order, with the dense path's metric check before anything about the set.
+static hx_status dense_restricted_host(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
+                                       const uint64_t* cand_ids, size_t n_cand, const hx_candidates* set, bool is_set,
+                                       uint64_t* out_ids, float* out_scores, uint32_t* out_counts, hx_stats* stats) {
+  if (!ix) {
+    hx_set_error("null index handle");
+    return HX_ERR_INDEX_NOT_FOUND;
+  }
+  uint32_t k, ef;
+  hx_status rc = check_params(ix, p, &k, &ef);
+  if (rc) return rc;
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (B == 0) return HX_OK;
+  if (!queries || !out_ids || !out_scores || !out_counts || (is_set ? !set : (n_cand && !cand_ids))) return HX_ERR_INVALID_PARAMETER;
+  if (ix->cfg.metric == HX_METRIC_MANHATTAN) {
+    hx_set_error("the L1 metric is not a contraction: use hx_search_restricted");
+    return HX_ERR_UNSUPPORTED;
+  }
+  const uint64_t n = is_set ? set->n : n_cand;
+  if (n > 1000000ull) {
+    hx_set_error("restricted vector search accepts at most 1000000 unique candidates");
+    return HX_ERR_QUERY;
+  }
+  if (n == 0) {   // RestrictedVectorCandidates::Empty => Ok(vec![]) before any I/O
+    for (size_t b = 0; b < B; ++b) out_counts[b] = 0;
+    return HX_OK;
+  }
+  if (std::min<uint64_t>(k, n) > 800) {
+    hx_set_error("restricted vector search result count must be at most 800, got %llu",
+                 (unsigned long long)std::min<uint64_t>(k, n));
+    return HX_ERR_QUERY;
+  }
+  if (!is_set)
+    for (uint64_t i = 1; i < n; ++i)
+      if (cand_ids[i] <= cand_ids[i - 1]) {
+        hx_set_error("candidate ids must be ascending and unique (RoaringTreemap iteration order); position %llu",
+                     (unsigned long long)i);
+        return HX_ERR_INVALID_PARAMETER;
+      }
+  if (is_set && (set->ix != ix || set->generation != ix->vector_generation)) {
+    hx_set_error("candidate set does not belong to this index image (vectors were reloaded or deleted?)");
+    return HX_ERR_INVARIANT_VIOLATION;
+  }
+  HX_CUDA(cudaSetDevice(ix->device));
+  if (ix->n == 0 || !ix->populated) return answer_empty_index(ix, queries, B, out_counts, nullptr);
+  HxScratch* s = nullptr;
+  if ((rc = hx_acquire_scratch(ix, &s))) return rc;
+  ScratchGuard guard{ix, s};
+  uint32_t launches = 0;
+  if ((rc = stage_queries(ix, s, queries, B, &launches))) return rc;
+  const uint32_t* slots = nullptr;
+  if (is_set) {
+    slots = set->d_slots;
+  } else {
+    if ((rc = s->d_cand_ids.reserve(n)) || (rc = s->d_cand_slots.reserve(n))) return rc;
+    HX_CUDA(cudaMemcpyAsync(s->d_cand_ids.p, cand_ids, n * sizeof(uint64_t), cudaMemcpyHostToDevice, s->stream));
+    k_map_candidates<<<(unsigned)((n + 255) / 256), 256, 0, s->stream>>>(
+        ix->d_ids, (uint32_t)ix->n, s->d_cand_ids.p, n, s->d_cand_slots.p, ix->contiguous ? 1 : 0, ix->first_id, ix->d_deleted);
+    HX_CUDA(cudaGetLastError());
+    launches++;
+    slots = s->d_cand_slots.p;
+  }
+  const uint32_t* d_present = nullptr;
+  size_t present = 0;
+  if ((rc = hx_dense_compact(ix, s, slots, n, s->stream, &d_present, &present, &launches))) return rc;
+  if ((rc = s->d_out_ids.reserve(B * (size_t)k)) || (rc = s->d_out_scores.reserve(B * (size_t)k)) ||
+      (rc = s->d_out_counts.reserve(B)))
+    return rc;
+  // below the dense path's minimum the exact scan over the same slot list: hx_search_restricted's answer and launches
+  const bool dense = present >= hx_dense_min_rows(k);
+  if (dense)
+    rc = hx_dense_restricted_device(ix, s, s->d_queries.p, B, k, d_present, present, s->d_out_ids.p, s->d_out_scores.p,
+                                    s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches);
+  else
+    rc = launch_scan_select(ix, s, s->d_queries.p, B, k, slots, nullptr, true, n, n, (uint64_t)B * n, s->d_out_ids.p,
+                            s->d_out_scores.p, s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches);
+  if (rc) return rc;
+  if ((rc = s->h_status.reserve(B)) || (rc = s->h_err.reserve(1))) return rc;
+  HX_CUDA(cudaMemcpyAsync(out_ids, s->d_out_ids.p, B * (size_t)k * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaMemcpyAsync(out_scores, s->d_out_scores.p, B * (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaMemcpyAsync(out_counts, s->d_out_counts.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaMemcpyAsync(s->h_status.p, s->d_qstatus.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaMemcpyAsync(s->h_err.p, s->d_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaStreamSynchronize(s->stream));
+  for (size_t b = 0; b < B; ++b)
+    if (s->h_status.p[b] != HX_ST_OK) return status_from_word(s->h_status.p[b], b, "query");
+  if ((rc = check_device_flags(s->h_err.p[0]))) return rc;
+  float ms = 0.f;
+  if (cudaEventElapsedTime(&ms, s->ev0, s->ev1) == cudaSuccess) {   // k_dense_scores, or the exact scan below the minimum
+    ix->last_kernel_ms = ms;
+    ix->last_kernel_launches = 1;
+  }
+  if (stats) {
+    const uint64_t dim = ix->cfg.dimension, ldb = (dim + 63) / 64 * 64;
+    stats->kernel_launches = launches;
+    if (dense) {
+      stats->distance_computations = (uint64_t)B * present;
+      // gather (f32 rows in, bf16 tile and row terms out), then the tile read once by the contraction
+      stats->algorithmic_bytes = present * (4 * dim + 2 * ldb + 4) + present * 2 * ldb;
+      stats->reserved = (uint64_t)(2.0 * (double)B * (double)present * (double)ldb);   // flop of the contraction
+    } else {
+      stats->distance_computations = (uint64_t)B * n;
+      stats->vectors_loaded = (uint64_t)B * n;
+      stats->algorithmic_bytes = (uint64_t)B * n * (4 * dim + (ix->cfg.metric == HX_METRIC_COSINE ? 4 : 0));
+    }
+  }
+  return HX_OK;
+}
+
+extern "C" hx_status hx_search_dense_restricted(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
+                                                const uint64_t* cand_ids, size_t n_cand, uint64_t* out_ids,
+                                                float* out_scores, uint32_t* out_counts, hx_stats* stats) {
+  return dense_restricted_host(ix, queries, B, p, cand_ids, n_cand, nullptr, false, out_ids, out_scores, out_counts, stats);
+}
+
+extern "C" hx_status hx_search_dense_restricted_set(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
+                                                    const hx_candidates* set, uint64_t* out_ids, float* out_scores,
+                                                    uint32_t* out_counts, hx_stats* stats) {
+  return dense_restricted_host(ix, queries, B, p, nullptr, 0, set, true, out_ids, out_scores, out_counts, stats);
+}
+
 // ------------------------------------------------------------------------------------------------
 // SimHash policy mode (search.rs:595-992, policy.rs) — the production-default SearchParams
 // ------------------------------------------------------------------------------------------------

@@ -236,3 +236,11 @@ hx_status hx_dense_impl(hx_index* ix, const float* queries, size_t B, const hx_s
 hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
                           uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
                           cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out);
+// rows below which the dense paths answer with the exact scan (the tensor-core pass could not fill its nominee lists)
+size_t hx_dense_min_rows(uint32_t k);
+hx_status hx_dense_compact(hx_index* ix, HxScratch* scr, const uint32_t* d_slots, size_t n, cudaStream_t stream,
+                           const uint32_t** d_present, size_t* n_present, uint32_t* launches);
+hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k,
+                                     const uint32_t* d_present, size_t n_present, uint64_t* d_out_ids, float* d_out_sc,
+                                     uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1,
+                                     uint32_t* launches);

@@ -371,6 +371,73 @@ __global__ void __launch_bounds__(HXD_SORT_THREADS) k_nominee_slots(const uint64
   }
 }
 
+// ---- order-preserving compaction of a candidate slot list (hx_search_dense_restricted) ----------------------------------------
+// Drops the HX_ABSENT entries (ids without a row, deleted rows) of an ascending slot list and keeps the rest in order, so
+// that the gathered tile holds present rows only: an absent row left in the tile would take a column and bucket space and
+// could leave the count short of min(k, present).  Two launches: per-tile counts, then each tile sums the counts before it
+// and scatters.  Tile = HXD_CPT_ROWS rows of 256 slots; row r of a tile is slots [256 r, 256 r + 256), one per thread, so
+// the loads are coalesced and a present slot's rank is (rank of its warp within the row, ballot prefix within the warp).
+#define HXD_CPT_THREADS 256
+#define HXD_CPT_ROWS 16
+#define HXD_CPT_TILE (HXD_CPT_THREADS * HXD_CPT_ROWS)
+
+__global__ void __launch_bounds__(HXD_CPT_THREADS) k_compact_count(const uint32_t* __restrict__ slots, size_t n,
+                                                                  uint32_t* __restrict__ tile_counts) {
+  __shared__ uint32_t ws[HXD_CPT_THREADS / 32];
+  const size_t t0 = (size_t)blockIdx.x * HXD_CPT_TILE;
+  uint32_t c = 0;
+#pragma unroll
+  for (int r = 0; r < HXD_CPT_ROWS; ++r) {
+    const size_t i = t0 + (size_t)r * HXD_CPT_THREADS + threadIdx.x;
+    c += i < n && slots[i] != HX_ABSENT;
+  }
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31u) == 0) ws[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t s = 0;
+    for (int w = 0; w < HXD_CPT_THREADS / 32; ++w) s += ws[w];
+    tile_counts[blockIdx.x] = s;
+  }
+}
+
+__global__ void __launch_bounds__(HXD_CPT_THREADS) k_compact_scatter(const uint32_t* __restrict__ slots, size_t n,
+                                                                    const uint32_t* __restrict__ tile_counts,
+                                                                    uint32_t* __restrict__ out, uint32_t* __restrict__ out_count) {
+  __shared__ uint32_t ws[HXD_CPT_THREADS / 32];
+  __shared__ uint32_t off[HXD_CPT_ROWS * (HXD_CPT_THREADS / 32)];   // output offsets of the (row, warp) groups, in that order
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const size_t t0 = (size_t)blockIdx.x * HXD_CPT_TILE;
+  // present slots of the tiles before this one
+  uint32_t base = 0;
+  for (uint32_t t = threadIdx.x; t < blockIdx.x; t += HXD_CPT_THREADS) base += tile_counts[t];
+  base = __reduce_add_sync(0xffffffffu, base);
+  if (lane == 0) ws[warp] = base;
+  uint32_t v[HXD_CPT_ROWS], mask[HXD_CPT_ROWS];
+#pragma unroll
+  for (int r = 0; r < HXD_CPT_ROWS; ++r) {
+    const size_t i = t0 + (size_t)r * HXD_CPT_THREADS + threadIdx.x;
+    v[r] = i < n ? slots[i] : HX_ABSENT;
+    mask[r] = __ballot_sync(0xffffffffu, v[r] != HX_ABSENT);
+    if (lane == 0) off[r * (HXD_CPT_THREADS / 32) + warp] = __popc(mask[r]);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t s = 0;
+    for (int w = 0; w < HXD_CPT_THREADS / 32; ++w) s += ws[w];
+    for (int j = 0; j < HXD_CPT_ROWS * (HXD_CPT_THREADS / 32); ++j) {
+      const uint32_t c = off[j];
+      off[j] = s;
+      s += c;
+    }
+    if (blockIdx.x == gridDim.x - 1) *out_count = s;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int r = 0; r < HXD_CPT_ROWS; ++r)
+    if (v[r] != HX_ABSENT) out[off[r * (HXD_CPT_THREADS / 32) + warp] + __popc(mask[r] & ((1u << lane) - 1u))] = v[r];
+}
+
 // ---- host ------------------------------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -548,31 +615,34 @@ static hx_status dense_exact_scan(hx_index* ix, HxScratch* scr, const float* d_q
   return HX_OK;
 }
 
-// Everything below is enqueued on `stream`; nothing synchronises with the host (buffers, tensor maps and the nominee
-// offsets are cached in the scratch set across calls).  d_queries: B x dim f32 on the device.  Per-query validation status
-// is left in s->d_qstatus (a query that fails validation yields count 0); error flags accumulate in s->d_err[0].
-hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
-                          uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
-                          cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out) {
-  hx_status rc = dense_check(ix, p);
-  if (rc) return rc;
-  if (B == 0) return HX_OK;
-  if (ix->n == 0 || !ix->populated) {
-    HX_CUDA(cudaMemsetAsync(d_out_cnt, 0, B * sizeof(uint32_t), stream));
-    return HX_OK;
-  }
-  const uint32_t dim = ix->cfg.dimension, k = p->k;
+// Small corpora get the exact scan.  The tensor-core pass hands each query at most HXD_PARTS * HXD_T = 32 nominees per run
+// of tiles, and a run is at least one 256-row tile, so a corpus of few tiles cannot fill k' = min(max(4k, 64), 800, rows)
+// nominees, and its count could fall short of min(k, rows).  From 8 * min(max(4k, 64), 800) rows on, every run but the
+// last holds a full tile (32 nominees), which covers k' (n_split below is at least k'/4 runs or every tile).  Below that
+// the exact scan costs at most 6400 rows per query.
+size_t hx_dense_min_rows(uint32_t k) { return 8 * (size_t)std::min<uint32_t>(std::max<uint32_t>(4 * k, 64), 800); }
+
+// The corpus a tensor-core pass runs over: `n` bf16 rows in tile placement (k_to_bf16 with tiled = 1), their row terms
+// (indexed by position), and the ascending slot table that maps row w of the view to its corpus slot.
+struct HxDenseView {
+  const void* rows;
+  const float* aux;
+  const uint32_t* slots;
+  size_t n;
+};
+
+// Tensor-core nomination over the view, then the exact re-rank with the reference arithmetic.  Needs
+// n >= hx_dense_min_rows(k) and k <= 800, and the queries' exact headers and status words in scr->d_qhdr / d_qstatus.
+// Everything is enqueued on `stream`; nothing synchronises with the host (buffers, the query tensor map and the nominee
+// offsets are cached in the scratch set across calls; the corpus map is keyed on the view's (base, rows)).
+static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxDenseView& v,
+                            uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0,
+                            cudaEvent_t e1, uint32_t* launches_out) {
+  hx_status rc;
+  const uint32_t dim = ix->cfg.dimension;
   const uint32_t ldb = (dim + HXD_BK - 1) / HXD_BK * HXD_BK;
-  if ((rc = ensure_dense_state(ix, ldb, false, stream))) return rc;
-  const size_t n = ix->n_live;   // rows of the bf16 copy: the live rows, compacted
-  // Small corpora get the exact scan over every live row.  The tensor-core pass hands each query at most
-  // HXD_PARTS * HXD_T = 32 nominees per run of tiles, and a run is at least one 256-row tile, so a corpus of few tiles
-  // cannot fill k' = min(max(4k, 64), 800, live rows) nominees, and its count could fall short of min(k, live rows).
-  // From 8 * min(max(4k, 64), 800) live rows on, every run but the last holds a full tile (32 nominees), which covers k'
-  // (n_split below is at least k'/4 runs or every tile).  Below that the exact scan costs at most 6400 rows per query.
+  const size_t n = v.n;
   const uint32_t kcap = std::min<uint32_t>(std::max<uint32_t>(4 * k, 64), 800);
-  if (n < 8 * (size_t)kcap) return dense_exact_scan(ix, scr, d_q, B, p, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out);
-  if ((rc = ensure_dense_state(ix, ldb, true, stream))) return rc;
   const uint32_t m_tiles = (uint32_t)((B + HXD_BM - 1) / HXD_BM), n_tiles = (uint32_t)((n + HXD_BN - 1) / HXD_BN);
   const size_t B_pad = (size_t)m_tiles * HXD_BM, n_pad = (size_t)n_tiles * HXD_BN;
   const size_t n_ctas = (size_t)std::max(1, ix->sm_count);   // one persistent CTA per SM
@@ -624,15 +694,14 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
     dc.kprime = kprime;
     dc.ldb = ldb;
   }
-  if (dc.map_x_base != ix->d_vec_bf16 || dc.map_x_rows != n_pad) {
-    if ((rc = make_map(reinterpret_cast<CUtensorMap*>(dc.map_x), ix->d_vec_bf16, n_pad, ldb, HXD_BH))) return rc;   // one MMA tile = half a placement tile
-    dc.map_x_base = ix->d_vec_bf16;
+  if (dc.map_x_base != v.rows || dc.map_x_rows != n_pad) {
+    if ((rc = make_map(reinterpret_cast<CUtensorMap*>(dc.map_x), const_cast<void*>(v.rows), n_pad, ldb, HXD_BH))) return rc;   // one MMA tile = half a placement tile
+    dc.map_x_base = v.rows;
     dc.map_x_rows = n_pad;
   }
   uint32_t launches = 0;
-  dense_validate(ix, d_q, B, d_qhdr, d_status, stream);
   k_to_bf16<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(d_q, B, dim, dim, d_qb, ldb, d_qaux, ix->cfg.metric, 0, nullptr);
-  launches += 2;
+  launches += 1;
   HX_CUDA(cudaGetLastError());
   // ---- tensor-core pass ----
   HxDenseArgs a{};
@@ -642,7 +711,7 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
   a.m_tiles = m_tiles;
   a.n_tiles = n_tiles;
   a.n_split = n_split;
-  a.row_aux = ix->d_sqnorm;
+  a.row_aux = v.aux;
   a.q_aux = d_qaux;
   a.keys = d_keys;
   a.metric = ix->cfg.metric;
@@ -675,7 +744,7 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
   uint32_t width = 32;
   while (width < kprime) width <<= 1;
   k_nominee_slots<<<(unsigned)std::min<size_t>(B, 65535), HXD_SORT_THREADS, 0, stream>>>(d_sel_ids, B, kprime, width,
-                                                                                       ix->d_live_slots, d_cslots);
+                                                                                       v.slots, d_cslots);
   launches += 2;
   HxScanArgs sa{};
   sa.queries = d_q;
@@ -711,6 +780,82 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
   launches += 2;
   HX_CUDA(cudaGetLastError());
   if (launches_out) *launches_out = launches;
+  return HX_OK;
+}
+
+// hx_search_dense over every live row.  Everything below is enqueued on `stream`; nothing synchronises with the host once
+// the dense state exists.  d_queries: B x dim f32 on the device.  Per-query validation status is left in s->d_qstatus
+// (a query that fails validation yields count 0); error flags accumulate in s->d_err[0].
+hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
+                          uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
+                          cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out) {
+  hx_status rc = dense_check(ix, p);
+  if (rc) return rc;
+  if (B == 0) return HX_OK;
+  if (ix->n == 0 || !ix->populated) {
+    HX_CUDA(cudaMemsetAsync(d_out_cnt, 0, B * sizeof(uint32_t), stream));
+    return HX_OK;
+  }
+  const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
+  if ((rc = ensure_dense_state(ix, ldb, false, stream))) return rc;
+  const size_t n = ix->n_live;   // rows of the bf16 copy: the live rows, compacted
+  if (n < hx_dense_min_rows(p->k))
+    return dense_exact_scan(ix, scr, d_q, B, p, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out);
+  if ((rc = ensure_dense_state(ix, ldb, true, stream))) return rc;
+  if ((rc = scr->d_qhdr.reserve(B)) || (rc = scr->d_qstatus.reserve(B))) return rc;
+  dense_validate(ix, d_q, B, scr->d_qhdr.p, scr->d_qstatus.p, stream);
+  const HxDenseView v{ix->d_vec_bf16, ix->d_sqnorm, ix->d_live_slots, n};
+  rc = dense_pass(ix, scr, d_q, B, p->k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out);
+  if (!rc && launches_out) *launches_out += 1;
+  return rc;
+}
+
+// hx_search_dense_restricted, step 1: the present entries of the ascending candidate slot list `d_slots` (n entries,
+// HX_ABSENT for ids without a row and for deleted rows), compacted in order into scratch.  Synchronises the stream to read
+// the count back (4 bytes).
+hx_status hx_dense_compact(hx_index* ix, HxScratch* scr, const uint32_t* d_slots, size_t n, cudaStream_t stream,
+                           const uint32_t** d_present, size_t* n_present, uint32_t* launches) {
+  hx_status rc;
+  const size_t tiles = (n + HXD_CPT_TILE - 1) / HXD_CPT_TILE;
+  if ((rc = scr->misc[11].reserve(n * 4)) || (rc = scr->misc[12].reserve((tiles + 1) * 4)) || (rc = scr->h_err.reserve(1)))
+    return rc;
+  uint32_t* out = reinterpret_cast<uint32_t*>(scr->misc[11].p);
+  uint32_t* counts = reinterpret_cast<uint32_t*>(scr->misc[12].p);   // [tiles] per-tile counts, then the total
+  k_compact_count<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(d_slots, n, counts);
+  k_compact_scatter<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(d_slots, n, counts, out, counts + tiles);
+  HX_CUDA(cudaGetLastError());
+  *launches += 2;
+  HX_CUDA(cudaMemcpyAsync(scr->h_err.p, counts + tiles, 4, cudaMemcpyDeviceToHost, stream));
+  HX_CUDA(cudaStreamSynchronize(stream));
+  *d_present = out;
+  *n_present = scr->h_err.p[0];
+  return HX_OK;
+}
+
+// hx_search_dense_restricted, step 2 (n_present >= hx_dense_min_rows(k)): the present rows, converted from the f32 rows into
+// a bf16 tile of this scratch set's own (k_to_bf16: tile placement over candidate RANK, cosine power-of-two scaling, row
+// terms), then the tensor-core pass over that tile with the compacted slots as its slot table.  The whole-corpus bf16 copy
+// is neither built nor read.  The queries' headers and status words must be in scr->d_qhdr / d_qstatus.
+hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k,
+                                     const uint32_t* d_present, size_t n_present, uint64_t* d_out_ids, float* d_out_sc,
+                                     uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1,
+                                     uint32_t* launches) {
+  hx_status rc;
+  const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
+  const size_t n_pad = (n_present + HXD_BN - 1) / HXD_BN * HXD_BN;
+  if ((rc = scr->misc[9].reserve(n_pad * (size_t)ldb * 2)) || (rc = scr->misc[10].reserve(n_pad * 4))) return rc;
+  void* tile = scr->misc[9].p;
+  float* aux = reinterpret_cast<float*>(scr->misc[10].p);
+  // the positions of the last placement tile that no candidate fills read as zero rows
+  HX_CUDA(cudaMemsetAsync(static_cast<unsigned char*>(tile) + (n_pad - HXD_BN) * (size_t)ldb * 2, 0, (size_t)HXD_BN * ldb * 2,
+                          stream));
+  k_to_bf16<<<(unsigned)((n_present + 7) / 8), 256, 0, stream>>>(ix->d_vec, n_present, ix->cfg.dimension, ix->ld,
+                                                                 (__nv_bfloat16*)tile, ldb, aux, ix->cfg.metric, 1, d_present);
+  HX_CUDA(cudaGetLastError());
+  const HxDenseView v{tile, aux, d_present, n_present};
+  uint32_t pass_launches = 0;
+  if ((rc = dense_pass(ix, scr, d_q, B, k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, &pass_launches))) return rc;
+  *launches += 1 + pass_launches;
   return HX_OK;
 }
 

@@ -505,6 +505,29 @@ hx_status hx_shard_group_last_ms(hx_shard_group* g, float* local_ms, float* coll
 hx_status hx_search_dense(hx_index* idx, const float* queries, size_t B, const hx_search_params* p,
                           uint64_t* out_ids, float* out_scores, uint32_t* out_counts,
                           hx_stats* stats);
+/* The same path restricted to ONE candidate set C shared by the B queries (prefiltered search as a contraction):
+ * hx_search_dense's contract over the rows of C that are present and not deleted.  Every score is the exact fp32 score,
+ * results are in (score, id) order with exact ties resolved by id, the count is min(k, |C ∩ live rows|), and ids without a
+ * row are never returned.  Per call the present rows of C are converted from the f32 rows into a bf16 tile (the
+ * whole-corpus bf16 copy is neither built nor read, so cfg.storage may be 0; the answer is the same at 0 and 1), the
+ * tensor cores nominate, and the exact kernel re-ranks.  Below 8 * min(max(4k, 64), 800) present rows the call runs the
+ * exact scan instead and returns hx_search_restricted's answer bit for bit.
+ * Admission, in order: params (as hx_search_restricted); B == 0 => HX_OK; null pointers => HX_ERR_INVALID_PARAMETER;
+ * Manhattan => HX_ERR_UNSUPPORTED; |C| > 1e6 => HX_ERR_QUERY; |C| == 0 => counts 0 (no query validation, no device work);
+ * min(k, |C|) > 800 => HX_ERR_QUERY (k is clamped to |C|; out_ids / out_scores are still B*k); ids not ascending and
+ * unique => HX_ERR_INVALID_PARAMETER; a set of another index or of an older vector generation => HX_ERR_INVARIANT_VIOLATION;
+ * empty or unpopulated index => counts 0 after query validation; then the queries are validated (first failing query's code).
+ * Device memory, held by the call's scratch set across calls: about present * (2 * ldb + 4) bytes for the tile (ldb = the
+ * dimension rounded up to 64) plus at most 16 bytes per candidate id and the nominee keys; about 1.5 GB at |C| = 1e6,
+ * d = 768.
+ * Per-query candidate sets stay on hx_search_restricted_multi / hx_search_restricted_sets. */
+hx_status hx_search_dense_restricted(hx_index* idx, const float* queries, size_t B, const hx_search_params* p,
+                                     const uint64_t* cand_ids, size_t n_cand, uint64_t* out_ids, float* out_scores,
+                                     uint32_t* out_counts, hx_stats* stats);
+/* Same with a device-resident set (hx_candidates_create): no ids cross PCIe. */
+hx_status hx_search_dense_restricted_set(hx_index* idx, const float* queries, size_t B, const hx_search_params* p,
+                                         const hx_candidates* set, uint64_t* out_ids, float* out_scores,
+                                         uint32_t* out_counts, hx_stats* stats);
 
 /* ---- SimHash filtering / sampling policy: the production-default search mode ------------------------------
  * SearchParams::new(k) is SimHashMode::Adaptive: layer 0 then runs Layer0Policy::decide per expansion
