@@ -190,6 +190,7 @@ ABI_SYMBOLS = [
     "hx_index_load_upper_vector_rows", "hx_index_set_version", "hx_index_get_version", "hx_index_build_ex",
     "hx_filtered_budgets", "hx_search_filtered_graph", "hx_index_get_tuning", "hx_index_set_tuning",
     "hx_search_dense_restricted", "hx_search_dense_restricted_set",
+    "hx_search_dense_exact", "hx_search_dense_restricted_exact", "hx_search_dense_restricted_exact_set",
 ]
 
 _lib = None
@@ -258,6 +259,14 @@ def load_library():
                                              C.POINTER(SearchStats)]
     L.hx_search_dense_restricted_set.restype = C.c_int32
     L.hx_search_dense_restricted_set.argtypes = [vp, fp, sz, C.POINTER(_Params), vp, u64p, fp, u32p, C.POINTER(SearchStats)]
+    L.hx_search_dense_exact.restype = C.c_int32
+    L.hx_search_dense_exact.argtypes = [vp, fp, sz, C.POINTER(_Params), u64p, fp, u32p, C.POINTER(C.c_uint8), C.POINTER(SearchStats)]
+    L.hx_search_dense_restricted_exact.restype = C.c_int32
+    L.hx_search_dense_restricted_exact.argtypes = [vp, fp, sz, C.POINTER(_Params), u64p, sz, u64p, fp, u32p, C.POINTER(C.c_uint8),
+                                                   C.POINTER(SearchStats)]
+    L.hx_search_dense_restricted_exact_set.restype = C.c_int32
+    L.hx_search_dense_restricted_exact_set.argtypes = [vp, fp, sz, C.POINTER(_Params), vp, u64p, fp, u32p, C.POINTER(C.c_uint8),
+                                                       C.POINTER(SearchStats)]
     L.hx_last_error.restype = C.c_char_p
     L.hx_last_error_index.restype = C.c_uint32
     L.hx_version.restype = C.c_char_p
@@ -1004,6 +1013,37 @@ class VectorIndex:
                                                   sc.ctypes.data_as(C.POINTER(C.c_float)),
                                                   cnt.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(st)))
         return ids, sc, cnt
+
+    # ---- exact tensor-core search: (ids, scores, counts, how); how per query: 0 certified, 1 rescanned, 2 exact scan ----
+    def _dense_exact(self, fn, queries, params: SearchParams, set_args, stats):
+        qa, qp = _f32(queries)
+        B = qa.size // (params.query_dimension or self.dim)
+        cp = params._c()
+        k = cp.k
+        ids = np.zeros((B, k), dtype=np.uint64)
+        sc = np.zeros((B, k), dtype=np.float32)
+        cnt = np.zeros(B, dtype=np.uint32)
+        how = np.zeros(B, dtype=np.uint8)
+        st = stats if stats is not None else SearchStats()
+        _ck(fn(self.h, qp, B, C.byref(cp), *set_args, ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+               sc.ctypes.data_as(C.POINTER(C.c_float)), cnt.ctypes.data_as(C.POINTER(C.c_uint32)),
+               how.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(st)))
+        return ids, sc, cnt, how
+
+    def search_dense_exact_batch(self, queries, params: SearchParams, stats=None):
+        """hx_search_dense_exact: hx_search_restricted's answer over every live id, through the tensor cores where the
+        certificate proves it and the exact scan for the queries it cannot."""
+        return self._dense_exact(self.L.hx_search_dense_exact, queries, params, (), stats)
+
+    def search_dense_restricted_exact_batch(self, queries, params: SearchParams, allowed: RestrictedVectorCandidates,
+                                            stats=None):
+        """hx_search_dense_restricted_exact: the same over one candidate set shared by every query."""
+        ca, cpnt = _u64(allowed.ids)
+        return self._dense_exact(self.L.hx_search_dense_restricted_exact, queries, params, (cpnt, ca.size), stats)
+
+    def search_dense_restricted_exact_sets(self, queries, params: SearchParams, device_set: "DeviceCandidates", stats=None):
+        """hx_search_dense_restricted_exact_set: the same with a device-resident set (cache_candidates)."""
+        return self._dense_exact(self.L.hx_search_dense_restricted_exact_set, queries, params, (device_set.h,), stats)
 
     # ---- device-buffer path (raw pointers, e.g. torch tensors' data_ptr()) ----
     def search_device(self, d_queries_ptr, B, params: SearchParams, d_ids_ptr, d_scores_ptr, d_counts_ptr,

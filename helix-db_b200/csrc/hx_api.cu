@@ -237,6 +237,8 @@ void HxScratch::destroy() {
   d_fg_stamps.release(); d_fg_epochs.release(); d_fg_bridge.release(); d_fg_elig.release(); d_fg_bits.release(); d_fg_seed.release();
   d_vtab.release(); d_vpool.release(); d_vbusy.release(); d_prof.release(); d_pstats.release(); d_qsim.release();
   for (auto& m : misc) m.release();
+  x_flag.release(); x_status.release(); x_counts.release(); x_how.release(); x_queries.release(); x_hdr.release();
+  x_scores.release(); x_ids.release(); h_x.release();
   h_ids.release(); h_cand_offsets.release(); h_scores.release(); h_queries.release(); h_qhdr.release();
   h_counts.release(); h_qstats.release(); h_status.release(); h_err.release(); h_avail.release();
   d_block.release(); h_block.release();
@@ -1827,8 +1829,11 @@ static hx_status launch_scan_select(hx_index* ix, HxScratch* s, const float* d_q
                                     const uint32_t* d_slots, const uint64_t* d_offsets, bool shared, uint64_t n_shared,
                                     uint64_t max_cands, uint64_t total_keys, uint64_t* d_out_ids, float* d_out_scores,
                                     uint32_t* d_out_counts, cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1,
-                                    uint32_t* launches, const HxSetRefs* sets = nullptr) {
+                                    uint32_t* launches, const HxSetRefs* sets = nullptr, const float* q_hdr = nullptr,
+                                    const uint32_t* q_status = nullptr) {
   hx_status rc;
+  if (!q_hdr) q_hdr = s->d_qhdr.p;   // headers / status words of the B queries (default: the call's staged queries)
+  if (!q_status) q_status = s->d_qstatus.p;
   if ((rc = s->d_err.reserve(1))) return rc;
   HX_CUDA(cudaMemsetAsync(s->d_err.p, 0, sizeof(uint32_t), stream));
   const HxDev dev = ix->dev();
@@ -1848,8 +1853,8 @@ static hx_status launch_scan_select(hx_index* ix, HxScratch* s, const float* d_q
     }
     HxScanArgs a{};
     a.queries = d_queries;
-    a.q_hdr = s->d_qhdr.p;
-    a.q_status = s->d_qstatus.p;
+    a.q_hdr = q_hdr;
+    a.q_status = q_status;
     a.B = (uint32_t)B;
     a.cand_slots = d_slots;
     a.cand_offsets = d_offsets;
@@ -1884,8 +1889,8 @@ static hx_status launch_scan_select(hx_index* ix, HxScratch* s, const float* d_q
   if ((rc = s->d_keys.reserve(total_keys))) return rc;
   HxScanArgs a{};
   a.queries = d_queries;
-  a.q_hdr = s->d_qhdr.p;
-  a.q_status = s->d_qstatus.p;
+  a.q_hdr = q_hdr;
+  a.q_status = q_status;
   a.B = (uint32_t)B;
   a.cand_slots = d_slots;
   a.cand_offsets = d_offsets;
@@ -1922,7 +1927,7 @@ static hx_status launch_scan_select(hx_index* ix, HxScratch* s, const float* d_q
   sa.keys = s->d_keys.p;
   sa.cand_slots = d_slots;
   sa.cand_offsets = d_offsets;
-  sa.q_status = s->d_qstatus.p;
+  sa.q_status = q_status;
   sa.B = (uint32_t)B;
   sa.k = k;
   sa.shared_set = shared ? 1u : 0u;
@@ -2289,11 +2294,88 @@ extern "C" hx_status hx_search_dense(hx_index* ix, const float* queries, size_t 
   return hx_dense_impl(ix, queries, B, p, out_ids, out_scores, out_counts, stats);
 }
 
+extern "C" hx_status hx_search_dense_exact(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
+                                           uint64_t* out_ids, float* out_scores, uint32_t* out_counts, uint8_t* out_how,
+                                           hx_stats* stats) {
+  if (!ix) return HX_ERR_INDEX_NOT_FOUND;
+  HX_CUDA(cudaSetDevice(ix->device));
+  return hx_dense_impl(ix, queries, B, p, out_ids, out_scores, out_counts, stats, true, out_how);
+}
+
+// rescan, step 1: flagged query j (query flagged[j] of the call) -> row j of a contiguous batch, with its header and status
+// word.  One warp per flagged query.
+static __global__ void k_dense_gather(const float* __restrict__ q, const float* __restrict__ hdr,
+                                      const uint32_t* __restrict__ status, const uint32_t* __restrict__ flagged, size_t F,
+                                      uint32_t dim, float* __restrict__ gq, float* __restrict__ ghdr,
+                                      uint32_t* __restrict__ gstatus) {
+  const size_t j = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31u;
+  if (j >= F) return;
+  const size_t b = flagged[j];
+  for (uint32_t i = lane; i < dim; i += 32) gq[j * dim + i] = q[b * dim + i];
+  if (lane == 0) {
+    ghdr[j] = hdr[b];
+    gstatus[j] = status[b];
+  }
+}
+
+// rescan, step 3: the exact answer of flagged query j replaces the output row of query flagged[j]
+static __global__ void k_dense_scatter(const uint64_t* __restrict__ gids, const float* __restrict__ gsc,
+                                       const uint32_t* __restrict__ gcnt, const uint32_t* __restrict__ flagged, size_t F,
+                                       uint32_t k, uint64_t* __restrict__ ids, float* __restrict__ sc, uint32_t* __restrict__ cnt) {
+  const size_t j = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31u;
+  if (j >= F) return;
+  const size_t b = flagged[j];
+  const uint32_t c = gcnt[j];
+  for (uint32_t i = lane; i < c; i += 32) {
+    ids[b * k + i] = gids[j * k + i];
+    sc[b * k + i] = gsc[j * k + i];
+  }
+  if (lane == 0) cnt[b] = c;
+}
+
+hx_status hx_dense_rescan(hx_index* ix, HxScratch* s, const float* d_q, uint32_t k, const uint32_t* slots,
+                          size_t n_view, const HxDenseCert& cert, uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt,
+                          cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches, size_t* n_flagged,
+                          uint32_t* err_before) {
+  hx_status rc;
+  if ((rc = s->h_x.reserve(2)) || (rc = s->d_err.reserve(1))) return rc;
+  HX_CUDA(cudaMemcpyAsync(s->h_x.p, cert.n_flagged, 4, cudaMemcpyDeviceToHost, stream));
+  HX_CUDA(cudaMemcpyAsync(s->h_x.p + 1, s->d_err.p, 4, cudaMemcpyDeviceToHost, stream));
+  HX_CUDA(cudaStreamSynchronize(stream));
+  const size_t F = s->h_x.p[0];
+  *n_flagged = F;
+  *err_before = s->h_x.p[1];
+  if (F == 0) return HX_OK;
+  const uint32_t dim = ix->cfg.dimension;
+  if ((rc = s->x_queries.reserve(F * (size_t)dim)) || (rc = s->x_hdr.reserve(F)) || (rc = s->x_status.reserve(F)) ||
+      (rc = s->x_ids.reserve(F * (size_t)k)) || (rc = s->x_scores.reserve(F * (size_t)k)) || (rc = s->x_counts.reserve(F)))
+    return rc;
+  const unsigned grid = (unsigned)((F + 7) / 8);
+  k_dense_gather<<<grid, 256, 0, stream>>>(d_q, s->d_qhdr.p, s->d_qstatus.p, cert.flagged, F, dim, s->x_queries.p,
+                                           s->x_hdr.p, s->x_status.p);
+  HX_CUDA(cudaGetLastError());
+  ++*launches;
+  if ((rc = launch_scan_select(ix, s, s->x_queries.p, F, k, slots, nullptr, true, n_view, n_view, (uint64_t)F * n_view,
+                               s->x_ids.p, s->x_scores.p, s->x_counts.p, stream, e0, e1, launches, nullptr, s->x_hdr.p,
+                               s->x_status.p)))
+    return rc;
+  k_dense_scatter<<<grid, 256, 0, stream>>>(s->x_ids.p, s->x_scores.p, s->x_counts.p, cert.flagged, F, k, d_out_ids, d_out_sc,
+                                            d_out_cnt);
+  HX_CUDA(cudaGetLastError());
+  ++*launches;
+  return HX_OK;
+}
+
 // The dense path over one candidate set shared by the B queries: host ids (`cand_ids`, n_cand) or a device set (`set`).
 // Admission is restricted_host's, in its order, with the dense path's metric check before anything about the set.
+// `exact` (hx_search_dense_restricted_exact[_set]): the certificate follows the re-rank and the queries it cannot clear are
+// rescanned over the present slots; out_how (may be null) as hx_search_dense_exact's.
 static hx_status dense_restricted_host(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
                                        const uint64_t* cand_ids, size_t n_cand, const hx_candidates* set, bool is_set,
-                                       uint64_t* out_ids, float* out_scores, uint32_t* out_counts, hx_stats* stats) {
+                                       uint64_t* out_ids, float* out_scores, uint32_t* out_counts, hx_stats* stats,
+                                       bool exact = false, uint8_t* out_how = nullptr) {
   if (!ix) {
     hx_set_error("null index handle");
     return HX_ERR_INDEX_NOT_FOUND;
@@ -2308,6 +2390,7 @@ static hx_status dense_restricted_host(hx_index* ix, const float* queries, size_
     hx_set_error("the L1 metric is not a contraction: use hx_search_restricted");
     return HX_ERR_UNSUPPORTED;
   }
+  if (exact && out_how) memset(out_how, 2, B);
   const uint64_t n = is_set ? set->n : n_cand;
   if (n > 1000000ull) {
     hx_set_error("restricted vector search accepts at most 1000000 unique candidates");
@@ -2360,20 +2443,29 @@ static hx_status dense_restricted_host(hx_index* ix, const float* queries, size_
     return rc;
   // below the dense path's minimum the exact scan over the same slot list: hx_search_restricted's answer and launches
   const bool dense = present >= hx_dense_min_rows(k);
+  HxDenseCert cert;
   if (dense)
     rc = hx_dense_restricted_device(ix, s, s->d_queries.p, B, k, d_present, present, s->d_out_ids.p, s->d_out_scores.p,
-                                    s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches);
+                                    s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches, exact ? &cert : nullptr);
   else
     rc = launch_scan_select(ix, s, s->d_queries.p, B, k, slots, nullptr, true, n, n, (uint64_t)B * n, s->d_out_ids.p,
                             s->d_out_scores.p, s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches);
   if (rc) return rc;
+  size_t flagged = 0;
+  uint32_t err_before = 0;
+  if (exact && dense &&
+      (rc = hx_dense_rescan(ix, s, s->d_queries.p, k, d_present, present, cert, s->d_out_ids.p, s->d_out_scores.p,
+                            s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches, &flagged, &err_before)))
+    return rc;
   if ((rc = s->h_status.reserve(B)) || (rc = s->h_err.reserve(1))) return rc;
+  if (exact && dense && out_how) HX_CUDA(cudaMemcpyAsync(out_how, cert.how, B, cudaMemcpyDeviceToHost, s->stream));
   HX_CUDA(cudaMemcpyAsync(out_ids, s->d_out_ids.p, B * (size_t)k * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
   HX_CUDA(cudaMemcpyAsync(out_scores, s->d_out_scores.p, B * (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
   HX_CUDA(cudaMemcpyAsync(out_counts, s->d_out_counts.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
   HX_CUDA(cudaMemcpyAsync(s->h_status.p, s->d_qstatus.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
   HX_CUDA(cudaMemcpyAsync(s->h_err.p, s->d_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
   HX_CUDA(cudaStreamSynchronize(s->stream));
+  s->h_err.p[0] |= err_before;
   for (size_t b = 0; b < B; ++b)
     if (s->h_status.p[b] != HX_ST_OK) return status_from_word(s->h_status.p[b], b, "query");
   if ((rc = check_device_flags(s->h_err.p[0]))) return rc;
@@ -2390,6 +2482,11 @@ static hx_status dense_restricted_host(hx_index* ix, const float* queries, size_
       // gather (f32 rows in, bf16 tile and row terms out), then the tile read once by the contraction
       stats->algorithmic_bytes = present * (4 * dim + 2 * ldb + 4) + present * 2 * ldb;
       stats->reserved = (uint64_t)(2.0 * (double)B * (double)present * (double)ldb);   // flop of the contraction
+      if (flagged) {   // the rescanned queries' full scans over the present rows
+        stats->distance_computations += flagged * present;
+        stats->vectors_loaded += flagged * present;
+        stats->algorithmic_bytes += flagged * present * (4 * dim + (ix->cfg.metric == HX_METRIC_COSINE ? 4 : 0));
+      }
     } else {
       stats->distance_computations = (uint64_t)B * n;
       stats->vectors_loaded = (uint64_t)B * n;
@@ -2409,6 +2506,22 @@ extern "C" hx_status hx_search_dense_restricted_set(hx_index* ix, const float* q
                                                     const hx_candidates* set, uint64_t* out_ids, float* out_scores,
                                                     uint32_t* out_counts, hx_stats* stats) {
   return dense_restricted_host(ix, queries, B, p, nullptr, 0, set, true, out_ids, out_scores, out_counts, stats);
+}
+
+extern "C" hx_status hx_search_dense_restricted_exact(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
+                                                      const uint64_t* cand_ids, size_t n_cand, uint64_t* out_ids,
+                                                      float* out_scores, uint32_t* out_counts, uint8_t* out_how,
+                                                      hx_stats* stats) {
+  return dense_restricted_host(ix, queries, B, p, cand_ids, n_cand, nullptr, false, out_ids, out_scores, out_counts, stats,
+                               true, out_how);
+}
+
+extern "C" hx_status hx_search_dense_restricted_exact_set(hx_index* ix, const float* queries, size_t B,
+                                                          const hx_search_params* p, const hx_candidates* set,
+                                                          uint64_t* out_ids, float* out_scores, uint32_t* out_counts,
+                                                          uint8_t* out_how, hx_stats* stats) {
+  return dense_restricted_host(ix, queries, B, p, nullptr, 0, set, true, out_ids, out_scores, out_counts, stats, true,
+                               out_how);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -117,6 +117,12 @@ struct HxScratch {
   bool prof_init = false;
   DevBuf<uint8_t> misc[16];   // dense path buffers (kept across calls)
   HxDenseCache dense;
+  // exact dense entries: certificate flags + compaction + the view word, how, and the gathered rescan queries and results
+  DevBuf<uint32_t> x_flag, x_status, x_counts;
+  DevBuf<uint8_t> x_how;
+  DevBuf<float> x_queries, x_hdr, x_scores;
+  DevBuf<uint64_t> x_ids;
+  PinBuf<uint32_t> h_x;
   DevBuf<uint8_t> d_block;    // small calls: results packed into one block -> one device-to-host copy
   PinBuf<uint8_t> h_block;
   PinBuf<uint64_t> h_ids, h_cand_offsets;
@@ -229,13 +235,31 @@ hx_status hx_launch_cta_ring(hx_index* ix, const HxCtaRingCfg& c, const HxHnswAr
                              cudaStream_t stream, int* ctas_per_sm);
 bool hx_slot_of(const hx_index* ix, uint64_t id, uint32_t* slot);
 
+// The certificate of the exact dense entries (k_dense.cu: k_dense_certify), left on the call's stream for the rescan
+struct HxDenseCert {
+  bool small = false;                   // the view is below hx_dense_min_rows(k): the exact scan answered every query
+  const uint32_t* flagged = nullptr;    // [B] the indices of the queries the certificate could not clear, ascending
+  const uint32_t* n_flagged = nullptr;  // device word: how many
+  const uint8_t* how = nullptr;         // [B] 0 certified, 1 flagged
+};
+
 // implemented in k_build.cu / k_dense.cu
 hx_status hx_build_impl(hx_index* ix, const uint16_t* levels, uint64_t seed, int sequential);
+// exact = false: hx_search_dense; true: hx_search_dense_exact (out_how may be null)
 hx_status hx_dense_impl(hx_index* ix, const float* queries, size_t B, const hx_search_params* p, uint64_t* out_ids,
-                        float* out_scores, uint32_t* out_counts, hx_stats* stats);
+                        float* out_scores, uint32_t* out_counts, hx_stats* stats, bool exact = false,
+                        uint8_t* out_how = nullptr);
+// cert != null: the certificate runs after the re-rank (or cert->small is set)
 hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
                           uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
-                          cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out);
+                          cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out, HxDenseCert* cert = nullptr);
+// hx_api.cu: the exact scan of the flagged queries over the view's ascending slot list, results scattered into the output
+// rows.  Synchronises the stream once to read the flagged count; *err_before receives the device error word as it was
+// before the scan reset it.
+hx_status hx_dense_rescan(hx_index* ix, HxScratch* s, const float* d_q, uint32_t k, const uint32_t* slots,
+                          size_t n_view, const HxDenseCert& cert, uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt,
+                          cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches, size_t* n_flagged,
+                          uint32_t* err_before);
 // rows below which the dense paths answer with the exact scan (the tensor-core pass could not fill its nominee lists)
 size_t hx_dense_min_rows(uint32_t k);
 hx_status hx_dense_compact(hx_index* ix, HxScratch* scr, const uint32_t* d_slots, size_t n, cudaStream_t stream,
@@ -243,4 +267,4 @@ hx_status hx_dense_compact(hx_index* ix, HxScratch* scr, const uint32_t* d_slots
 hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k,
                                      const uint32_t* d_present, size_t n_present, uint64_t* d_out_ids, float* d_out_sc,
                                      uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1,
-                                     uint32_t* launches);
+                                     uint32_t* launches, HxDenseCert* cert = nullptr);

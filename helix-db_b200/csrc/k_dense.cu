@@ -438,6 +438,139 @@ __global__ void __launch_bounds__(HXD_CPT_THREADS) k_compact_scatter(const uint3
     if (v[r] != HX_ABSENT) out[off[r * (HXD_CPT_THREADS / 32) + warp] + __popc(mask[r] & ((1u << lane) - 1u))] = v[r];
 }
 
+// ---- the certificate of the exact entries (hx_search_dense_exact, hx_search_dense_restricted_exact[_set]) ------------------
+// After the re-rank, query q's answer is exact unless a row the pass dropped belongs in it.  A dropped row r has approximate
+// score ŝ_r (a key of k_dense_scores) >= L_q, the smaller of
+//   * the tail (key HXD_T - 1) of every FULL bucket (tail != HX_KEY_MAX): a bucket keeps the HXD_T largest t and sc is
+//     monotone (non-increasing) in t, fmaxf clamp included, so every row it dropped has ŝ >= its tail;
+//   * the k'-th nominee's approximate score, when the first k_select kept k' keys (otherwise it dropped none).
+// With S_k the k-th exact score of the answer (the reference's fp32 bits), the query is certified iff
+//   floor(L_q) > S_k,   floor(L) = a lower bound on the reference's fp32 score of ANY row of the view with ŝ >= L,
+// i.e. L_q > S_k + E_q with E_q = L_q - floor(L_q).  floor is non-decreasing in L, so bounding at ŝ = L_q covers every
+// dropped row: each has exact score > S_k, so it is neither better than the k-th row nor tied with it.
+//
+// The bound (hxd_exact_floor; tests/test_dense_exact_reference.py restates it and checks it against the oracle).  Notation:
+// u = 2^-24 (fp32), u_b = 2^-8 (bf16: 8 significant bits), γ(n) = n u / (1 - n u), ldb = dim rounded up to 64.  q^, x^ are
+// the bf16 operands; Q = |q^|, X = |x^|.  Three error sources:
+//  (a) the pass's own fp32 arithmetic.  Tensor-core accumulation is not IEEE-specified; it is bounded as if every one of
+//      the ldb additions truncated (2^-23) and flushed anything below 2^-126 (inputs included):
+//        |s - <q^,x^>| <= c_acc Σ|q^_i x^_i| + 2 (ldb + 16) 2^-126 + 2^-126 Σ(|q^_i| + |x^_i|),  c_acc = (ldb + 16) 2^-22.
+//      The row / query terms are fp32 sums of exact bf16 squares, depth ldb/32 + 5: |qa - Q^2| <= γ_sq Q^2 + ldb 2^-150.
+//      Euclidean, sc = qa - fma(2, s, -ax) (two roundings, |operands| <= M = (Q + X)^2):
+//        |sc - |q^ - x^|^2| <= (γ_sq + c_acc + 3u) M + 2 ldb 2^-150 + 2 a_acc + 2^-150.
+//      Cosine, sc = 0.5 - 0.5 (s ax) qa with ax, qa = rsqrtf (2 ulp = 4u) of the sums; after k_to_bf16's power-of-two step
+//      every nonzero operand has its largest component in [1, 2), so Q, X >= 1 and every absolute term is relative:
+//        |sc - (1 - cos^)/2| <= 0.5 (c_acc + 1.01 Ψ) + 1.6u + 2^-100,  Ψ = 1.01 (2 ψ + u),  ψ = 1.01 (γ_sq + ldb 2^-150 + 4u).
+//      sc >= that error below the true value is all that is used: the clamp only raises ŝ, and the true value is >= 0.
+//  (b) bf16 rounding, in the distance domain, where it is a contraction.  |x^_i - x_i| <= u_b |x_i| + 2^-134 (bf16
+//      subnormal spacing 2^-133), so |x^ - x| <= u_b |x| + a, a = sqrt(ldb) 2^-134, and |x| <= (X + a) / (1 - u_b).
+//      Euclidean: D = |q - x| >= |q^ - x^| - |q^ - q| - |x^ - x| >= sqrt(ŝ - err) - β,
+//        β = u_b (Q + R + 2a) / (1 - u_b) + 2a,  R = an upper bound on X over the view (max of the row terms).
+//      Cosine: the score is |e_q - e_x|^2 / 4 over unit vectors e.  Scaling by 2^j changes no direction; rounding a vector
+//      w with |w^ - w| <= η |w| (η = u_b + sqrt(ldb) 2^-133, ldexpf's own rounding included) turns its direction by an
+//      angle whose chord is <= η' = 1.01 η / (1 - η).  So sqrt(score) >= sqrt(ŝ - err) - η'.  No norms enter.
+//  (c) the reference's fp32 score of the dropped row, since S_k is the reference's bits.  Euclidean: every term (q_i - x_i)^2
+//      is positive and sees at most 2 dim + 10 roundings (subtraction, fma chain, tree, scalar tail) plus at most that many
+//      underflows of 2^-150: s_ref >= (1 - γ(2 dim + 10)) D^2 - (2 dim + 10) 2^-150.  Cosine: the fast path runs only when
+//      |q||x| is a normal float, so the dot's underflow is another γ of |q||x|; with the norms' and the division's roundings
+//      |cos_ref - cos| <= 2 γ(2 dim + 10) + 6u, and 1 - cos plus the halving add 2u: |s_ref - s| <= 1.01 (γ + 3u) + 2u.  The
+//      f64 fallback is far more accurate than this.
+// Everything is evaluated in double with a relative margin of 2^-30 on the comparison.  A query is flagged — never
+// certified on an unproven bound — when its status word is not OK, its count is not k, S_k, L_q or the bound is not a
+// finite number (a NaN bound compares false), or (cosine) the query's or a row's fp32 norm is below FLT_MIN, where the
+// reference's own rounding of the norm is not relative (see k_dense_view_bound).
+#define HXD_U (1.0 / 16777216.0)
+__host__ __device__ inline double hxd_gamma(double n) { return n * HXD_U / (1.0 - n * HXD_U); }
+
+// lower bound on the reference's fp32 score of any row of the view whose approximate score is >= L (see above).
+// q_aux: the pass's query term (euclidean |q^|^2); r2: the largest row term of the view (euclidean |x^|^2)
+__host__ __device__ inline double hxd_exact_floor(int metric, uint32_t dim, uint32_t ldb, double L, double q_aux, double r2) {
+  const double u = HXD_U, ub = 1.0 / 256.0, sub = 0x1p-150, tiny = 0x1p-126, sd = sqrt((double)ldb);
+  const double c_acc = (ldb + 16.0) * 4.0 * u, g_sq = hxd_gamma(ldb / 32 + 5.0), n_ref = 2.0 * dim + 10.0;
+  if (metric == HXM_COSINE) {
+    const double psi = 1.01 * (g_sq + ldb * sub + 4.0 * u), Psi = 1.01 * (2.0 * psi + u);
+    const double err = 0.5 * (c_acc + 1.01 * Psi) + 1.6 * u + 0x1p-100;
+    const double eta = ub + sd * 0x1p-133, eta1 = 1.01 * eta / (1.0 - eta);
+    const double h = fmax(sqrt(fmax(L - err, 0.0)) - eta1, 0.0);   // <= half the chord between the true unit vectors
+    return h * h - (1.01 * (hxd_gamma(n_ref) + 3.0 * u) + 2.0 * u);
+  }
+  const double Q = sqrt((q_aux + ldb * sub) / (1.0 - g_sq)), X = sqrt((r2 + ldb * sub) / (1.0 - g_sq));
+  const double M = (Q + X) * (Q + X);
+  const double a_acc = 2.0 * (ldb + 16.0) * tiny + tiny * sd * (Q + X);
+  const double err = (g_sq + c_acc + 3.0 * u) * M + 2.0 * ldb * sub + 2.0 * a_acc + sub;
+  const double a = sd * 0x1p-134, beta = ub * (Q + X + 2.0 * a) / (1.0 - ub) + 2.0 * a;
+  const double D = fmax(sqrt(fmax(L - err, 0.0)) - beta, 0.0);   // <= |q - x|
+  return (1.0 - hxd_gamma(n_ref)) * D * D - n_ref * sub;
+}
+
+// What the bound needs from the whole view, one word; *out must be 0 before the launch.
+//   euclidean: the largest row term |x^|^2 over the positions that hold a row, as float bits (non-negative floats order
+//              like their bits): R^2;
+//   cosine:    1 when a row's exact header (its fp32 norm) is below FLT_MIN.  The reference's fast path divides by that
+//              norm, whose fp32 rounding is then not relative (a row of +-2^-149 has a norm 15% off), so part (c) of the
+//              bound does not hold for that row and no query of the call can be certified.
+__global__ void k_dense_view_bound(const float* __restrict__ aux, const float* __restrict__ hdr,
+                                   const uint32_t* __restrict__ slots, size_t n, int metric, uint32_t* __restrict__ out) {
+  const size_t n_pad = (n + HXD_BN - 1) / HXD_BN * HXD_BN;
+  uint32_t m = 0;
+  for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < n_pad; p += (size_t)gridDim.x * blockDim.x) {
+    if (metric == HXM_COSINE) {
+      if (p < n && !(hdr[slots[p]] >= FLT_MIN)) m = 1u;
+    } else if (p / HXD_BN * HXD_BN + hxd_row_at_pos((uint32_t)(p % HXD_BN)) < n) {
+      m = max(m, __float_as_uint(aux[p]));
+    }
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31u) == 0 && m) atomicMax(out, m);
+}
+
+struct HxCertArgs {
+  const uint64_t* keys;        // HxDensePassOut
+  uint32_t n_split, kprime;
+  const float* sel_sc;
+  const uint32_t* sel_cnt;
+  const float* q_aux;
+  const float* out_sc;         // [B][k] the re-ranked answer
+  const uint32_t* out_cnt;
+  const uint32_t* q_status;
+  const float* q_hdr;          // [B] exact query headers (cosine: fp32 norm)
+  const uint32_t* view_word;   // k_dense_view_bound's word
+  uint32_t B, k, dim, ldb;
+  int32_t metric;
+  uint32_t* flag;              // [B] q when the query must be rescanned, HX_ABSENT when certified (k_compact_* input)
+  uint8_t* how;                // [B] 0 certified, 1 rescanned
+};
+
+// one warp per query: the warp takes the minimum over its n_split * HXD_PARTS bucket tails, lane 0 decides
+__global__ void __launch_bounds__(256) k_dense_certify(HxCertArgs a) {
+  const size_t q = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31u;
+  if (q >= a.B) return;
+  const uint32_t nb = a.n_split * HXD_PARTS;
+  const uint64_t* kq = a.keys + q * nb * HXD_T;
+  uint32_t lb = 0x7f800000u;   // +inf: no full bucket
+  for (uint32_t i = lane; i < nb; i += 32) {
+    const uint64_t tail = kq[(size_t)i * HXD_T + HXD_T - 1];
+    if (tail != HX_KEY_MAX) lb = min(lb, (uint32_t)(tail >> 32));
+  }
+  lb = __reduce_min_sync(0xffffffffu, lb);
+  if (lane != 0) return;
+  float L = __uint_as_float(lb);
+  if (a.sel_cnt[q] == a.kprime) L = fminf(L, a.sel_sc[q * a.kprime + a.kprime - 1]);
+  bool ok = a.q_status[q] == 0u && a.out_cnt[q] == a.k;
+  const float sk = ok ? a.out_sc[q * a.k + a.k - 1] : 0.f;
+  ok = ok && isfinite(L) && isfinite(sk);
+  // cosine: the reference's norms of the query and of every row must be normal floats (k_dense_view_bound)
+  if (a.metric == HXM_COSINE) ok = ok && *a.view_word == 0u && a.q_hdr[q] >= FLT_MIN;
+  if (ok) {
+    const double r2 = a.metric == HXM_COSINE ? 0.0 : (double)__uint_as_float(*a.view_word);
+    const double lo = hxd_exact_floor(a.metric, a.dim, a.ldb, (double)L, (double)a.q_aux[q], r2);
+    ok = lo * (1.0 - 0x1p-30) > (double)sk;   // false for a NaN bound
+  }
+  a.flag[q] = ok ? HX_ABSENT : (uint32_t)q;
+  a.how[q] = ok ? 0 : 1;
+}
+
 // ---- host ------------------------------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -631,13 +764,24 @@ struct HxDenseView {
   size_t n;
 };
 
+// What a tensor-core pass leaves behind that bounds what it may have dropped (read by the certificate, k_dense_certify)
+struct HxDensePassOut {
+  const uint64_t* keys;      // [B][n_split][HXD_PARTS][HXD_T] bucket lists of k_dense_scores
+  uint32_t n_split;
+  const float* sel_sc;       // [B][kprime] approximate scores of the nominees, ascending
+  const uint32_t* sel_cnt;   // [B] nominees per query
+  uint32_t kprime;
+  const float* q_aux;        // [B] query terms of the pass (euclidean: |q^|^2)
+};
+
 // Tensor-core nomination over the view, then the exact re-rank with the reference arithmetic.  Needs
 // n >= hx_dense_min_rows(k) and k <= 800, and the queries' exact headers and status words in scr->d_qhdr / d_qstatus.
 // Everything is enqueued on `stream`; nothing synchronises with the host (buffers, the query tensor map and the nominee
 // offsets are cached in the scratch set across calls; the corpus map is keyed on the view's (base, rows)).
+// `pass_out` (may be null) receives the pass's internal buffers; they stay valid until the scratch set's next dense pass.
 static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxDenseView& v,
                             uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0,
-                            cudaEvent_t e1, uint32_t* launches_out) {
+                            cudaEvent_t e1, uint32_t* launches_out, HxDensePassOut* pass_out = nullptr) {
   hx_status rc;
   const uint32_t dim = ix->cfg.dimension;
   const uint32_t ldb = (dim + HXD_BK - 1) / HXD_BK * HXD_BK;
@@ -780,6 +924,57 @@ static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size
   launches += 2;
   HX_CUDA(cudaGetLastError());
   if (launches_out) *launches_out = launches;
+  if (pass_out) *pass_out = HxDensePassOut{d_keys, n_split, d_sel_sc, d_sel_cnt, kprime, d_qaux};
+  return HX_OK;
+}
+
+// The certificate after a pass over view `v` (see k_dense_certify), then the order-preserving compaction of the flagged
+// query indices.  Enqueued on `stream`, no synchronisation.  Buffers: the scratch set's x_flag / x_how, none of the pass's.
+static hx_status dense_certify(hx_index* ix, HxScratch* scr, size_t B, uint32_t k, const HxDenseView& v,
+                               const HxDensePassOut& po, const float* d_out_sc, const uint32_t* d_out_cnt, HxDenseCert* cert,
+                               cudaStream_t stream, uint32_t* launches) {
+  hx_status rc;
+  const size_t tiles = (B + HXD_CPT_TILE - 1) / HXD_CPT_TILE;
+  if ((rc = scr->x_flag.reserve(2 * B + tiles + 2)) || (rc = scr->x_how.reserve(B))) return rc;
+  uint32_t* flag = scr->x_flag.p;          // [B] per query
+  uint32_t* flagged = flag + B;            // [B] compacted
+  uint32_t* counts = flagged + B;          // [tiles] + the total
+  uint32_t* view_word = counts + tiles + 1;   // k_dense_view_bound
+  {
+    HX_CUDA(cudaMemsetAsync(view_word, 0, 4, stream));
+    const size_t n_pad = (v.n + HXD_BN - 1) / HXD_BN * HXD_BN;
+    const unsigned grid = (unsigned)std::min<size_t>((n_pad + 255) / 256, 4 * (size_t)std::max(1, ix->sm_count));
+    k_dense_view_bound<<<grid, 256, 0, stream>>>(v.aux, ix->d_hdr, v.slots, v.n, ix->cfg.metric, view_word);
+    ++*launches;
+  }
+  HxCertArgs a{};
+  a.keys = po.keys;
+  a.n_split = po.n_split;
+  a.kprime = po.kprime;
+  a.sel_sc = po.sel_sc;
+  a.sel_cnt = po.sel_cnt;
+  a.q_aux = po.q_aux;
+  a.out_sc = d_out_sc;
+  a.out_cnt = d_out_cnt;
+  a.q_status = scr->d_qstatus.p;
+  a.q_hdr = scr->d_qhdr.p;
+  a.view_word = view_word;
+  a.B = (uint32_t)B;
+  a.k = k;
+  a.dim = ix->cfg.dimension;
+  a.ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
+  a.metric = ix->cfg.metric;
+  a.flag = flag;
+  a.how = scr->x_how.p;
+  k_dense_certify<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(a);
+  k_compact_count<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(flag, B, counts);
+  k_compact_scatter<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(flag, B, counts, flagged, counts + tiles);
+  HX_CUDA(cudaGetLastError());
+  *launches += 3;
+  cert->small = false;
+  cert->flagged = flagged;
+  cert->n_flagged = counts + tiles;
+  cert->how = scr->x_how.p;
   return HX_OK;
 }
 
@@ -788,7 +983,7 @@ static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size
 // (a query that fails validation yields count 0); error flags accumulate in s->d_err[0].
 hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
                           uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
-                          cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out) {
+                          cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out, HxDenseCert* cert) {
   hx_status rc = dense_check(ix, p);
   if (rc) return rc;
   if (B == 0) return HX_OK;
@@ -799,14 +994,22 @@ hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t
   const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
   if ((rc = ensure_dense_state(ix, ldb, false, stream))) return rc;
   const size_t n = ix->n_live;   // rows of the bf16 copy: the live rows, compacted
-  if (n < hx_dense_min_rows(p->k))
+  if (n < hx_dense_min_rows(p->k)) {
+    if (cert) cert->small = true;
     return dense_exact_scan(ix, scr, d_q, B, p, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out);
+  }
   if ((rc = ensure_dense_state(ix, ldb, true, stream))) return rc;
   if ((rc = scr->d_qhdr.reserve(B)) || (rc = scr->d_qstatus.reserve(B))) return rc;
   dense_validate(ix, d_q, B, scr->d_qhdr.p, scr->d_qstatus.p, stream);
   const HxDenseView v{ix->d_vec_bf16, ix->d_sqnorm, ix->d_live_slots, n};
-  rc = dense_pass(ix, scr, d_q, B, p->k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out);
+  HxDensePassOut po{};
+  rc = dense_pass(ix, scr, d_q, B, p->k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out, cert ? &po : nullptr);
   if (!rc && launches_out) *launches_out += 1;
+  if (!rc && cert) {
+    uint32_t l = 0;
+    rc = dense_certify(ix, scr, B, p->k, v, po, d_out_sc, d_out_cnt, cert, stream, &l);
+    if (launches_out) *launches_out += l;
+  }
   return rc;
 }
 
@@ -839,7 +1042,7 @@ hx_status hx_dense_compact(hx_index* ix, HxScratch* scr, const uint32_t* d_slots
 hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k,
                                      const uint32_t* d_present, size_t n_present, uint64_t* d_out_ids, float* d_out_sc,
                                      uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1,
-                                     uint32_t* launches) {
+                                     uint32_t* launches, HxDenseCert* cert) {
   hx_status rc;
   const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
   const size_t n_pad = (n_present + HXD_BN - 1) / HXD_BN * HXD_BN;
@@ -854,20 +1057,27 @@ hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* 
   HX_CUDA(cudaGetLastError());
   const HxDenseView v{tile, aux, d_present, n_present};
   uint32_t pass_launches = 0;
-  if ((rc = dense_pass(ix, scr, d_q, B, k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, &pass_launches))) return rc;
+  HxDensePassOut po{};
+  if ((rc = dense_pass(ix, scr, d_q, B, k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, &pass_launches,
+                       cert ? &po : nullptr)))
+    return rc;
   *launches += 1 + pass_launches;
+  if (cert) return dense_certify(ix, scr, B, k, v, po, d_out_sc, d_out_cnt, cert, stream, launches);
   return HX_OK;
 }
 
 // Host-buffer entry point: a private stream + scratch set per call, the queries cross PCIe with one async copy, results
-// and per-query status come back with four, ONE stream synchronisation.
+// and per-query status come back with four, ONE stream synchronisation.  `exact` (hx_search_dense_exact): the certificate
+// follows the re-rank and the queries it cannot clear are rescanned (hx_dense_rescan: one more synchronisation, for the
+// flagged count); out_how (may be null) receives 0 / 1 per query, or 2 for every query when the exact scan answered all.
 hx_status hx_dense_impl(hx_index* ix, const float* queries, size_t B, const hx_search_params* p, uint64_t* out_ids,
-                        float* out_scores, uint32_t* out_counts, hx_stats* stats) {
+                        float* out_scores, uint32_t* out_counts, hx_stats* stats, bool exact, uint8_t* out_how) {
   hx_status rc = dense_check(ix, p);
   if (rc) return rc;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (B == 0) return HX_OK;
   if (!queries || !out_ids || !out_scores || !out_counts) return HX_ERR_INVALID_PARAMETER;
+  if (exact && out_how) memset(out_how, 2, B);
   if (ix->n == 0 || !ix->populated) {
     for (size_t b = 0; b < B; ++b) out_counts[b] = 0;
     return HX_OK;
@@ -883,15 +1093,25 @@ hx_status hx_dense_impl(hx_index* ix, const float* queries, size_t B, const hx_s
   cudaStream_t st = scr->stream;
   HX_CUDA(cudaMemcpyAsync(scr->d_queries.p, queries, B * (size_t)dim * 4, cudaMemcpyHostToDevice, st));
   uint32_t launches = 0;
+  HxDenseCert cert;
   if ((rc = hx_dense_device(ix, scr, scr->d_queries.p, B, p, scr->d_out_ids.p, scr->d_out_scores.p, scr->d_out_counts.p, st,
-                            scr->ev0, scr->ev1, &launches)))
+                            scr->ev0, scr->ev1, &launches, exact ? &cert : nullptr)))
+    return rc;
+  size_t flagged = 0;
+  uint32_t err_before = 0;
+  if (exact && !cert.small &&
+      (rc = hx_dense_rescan(ix, scr, scr->d_queries.p, k, ix->d_live_slots, ix->n_live, cert, scr->d_out_ids.p,
+                            scr->d_out_scores.p, scr->d_out_counts.p, st, scr->ev0, scr->ev1, &launches, &flagged,
+                            &err_before)))
     return rc;
   HX_CUDA(cudaMemcpyAsync(out_ids, scr->d_out_ids.p, B * (size_t)k * 8, cudaMemcpyDeviceToHost, st));
   HX_CUDA(cudaMemcpyAsync(out_scores, scr->d_out_scores.p, B * (size_t)k * 4, cudaMemcpyDeviceToHost, st));
   HX_CUDA(cudaMemcpyAsync(out_counts, scr->d_out_counts.p, B * 4, cudaMemcpyDeviceToHost, st));
   HX_CUDA(cudaMemcpyAsync(scr->h_status.p, scr->d_qstatus.p, B * 4, cudaMemcpyDeviceToHost, st));
   HX_CUDA(cudaMemcpyAsync(scr->h_err.p, scr->d_err.p, 4, cudaMemcpyDeviceToHost, st));
+  if (exact && !cert.small && out_how) HX_CUDA(cudaMemcpyAsync(out_how, cert.how, B, cudaMemcpyDeviceToHost, st));
   HX_CUDA(cudaStreamSynchronize(st));
+  scr->h_err.p[0] |= err_before;
   for (size_t b = 0; b < B; ++b)
     if (scr->h_status.p[b] != HX_ST_OK) {
       const uint32_t w = scr->h_status.p[b], code = w >> 24;
@@ -915,6 +1135,10 @@ hx_status hx_dense_impl(hx_index* ix, const float* queries, size_t B, const hx_s
     stats->distance_computations = (uint64_t)B * ix->n;
     stats->algorithmic_bytes = (uint64_t)ix->n * ldb * 2;   // corpus streamed once; the bound is the tensor pipe: 2*B*N*d flop
     stats->reserved = (uint64_t)(2.0 * (double)B * (double)ix->n * (double)ldb);   // flop of the contraction
+    if (flagged) {   // the rescanned queries' full scans
+      stats->distance_computations += flagged * ix->n_live;
+      stats->algorithmic_bytes += flagged * ix->n_live * (4ull * dim + (ix->cfg.metric == HX_METRIC_COSINE ? 4 : 0));
+    }
   }
   return HX_OK;
 }

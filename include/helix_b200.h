@@ -529,6 +529,27 @@ hx_status hx_search_dense_restricted_set(hx_index* idx, const float* queries, si
                                          const hx_candidates* set, uint64_t* out_ids, float* out_scores,
                                          uint32_t* out_counts, hx_stats* stats);
 
+/* Exact tensor-core search.  The answer of hx_search_restricted over every live id (resp. over C), bit for bit: ids, order,
+ * score bits and count, for every legal input.  After the re-rank a certificate bounds, per query, what the tensor-core pass
+ * may have dropped (bucket tails and the nominee cut, against the bf16 / fp32 error bound derived in csrc/k_dense.cu); a
+ * query it cannot prove exact is rescanned by the exact scan over every row of the view.  One more stream synchronisation
+ * than the entry of the same name (a 4-byte read-back of the flagged count); a rescanned query costs a full exact scan.
+ * out_how (B bytes, may be NULL): 0 = the tensor-core answer was certified, 1 = the query was rescanned because the
+ * certificate failed, 2 = the corpus / present set is below hx_dense_min_rows(k) = 8 * min(max(4k, 64), 800) rows and every
+ * query was answered by the exact scan outright (also for an empty index or set).  Admission and errors exactly as the
+ * entry of the same name without _exact.  hx_last_kernel_ms reports the rescan's scan kernel when queries were rescanned.
+ * hx_stats: kernel_launches includes the certificate, compaction, gather, scan and scatter; distance_computations and
+ * algorithmic_bytes add the rescanned queries' full scans. */
+hx_status hx_search_dense_exact(hx_index* idx, const float* queries, size_t B, const hx_search_params* p,
+                                uint64_t* out_ids, float* out_scores, uint32_t* out_counts, uint8_t* out_how,
+                                hx_stats* stats);
+hx_status hx_search_dense_restricted_exact(hx_index* idx, const float* queries, size_t B, const hx_search_params* p,
+                                           const uint64_t* cand_ids, size_t n_cand, uint64_t* out_ids, float* out_scores,
+                                           uint32_t* out_counts, uint8_t* out_how, hx_stats* stats);
+hx_status hx_search_dense_restricted_exact_set(hx_index* idx, const float* queries, size_t B, const hx_search_params* p,
+                                               const hx_candidates* set, uint64_t* out_ids, float* out_scores,
+                                               uint32_t* out_counts, uint8_t* out_how, hx_stats* stats);
+
 /* ---- SimHash filtering / sampling policy: the production-default search mode ------------------------------
  * SearchParams::new(k) is SimHashMode::Adaptive: layer 0 then runs Layer0Policy::decide per expansion
  * (policy.rs:119-175: adaptive collision threshold :576-597, adaptive sampling :558-574, pre-/post-sampling activation
