@@ -191,6 +191,7 @@ ABI_SYMBOLS = [
     "hx_filtered_budgets", "hx_search_filtered_graph", "hx_index_get_tuning", "hx_index_set_tuning",
     "hx_search_dense_restricted", "hx_search_dense_restricted_set",
     "hx_search_dense_exact", "hx_search_dense_restricted_exact", "hx_search_dense_restricted_exact_set",
+    "hx_candidates_make_resident", "hx_candidates_resident_bytes", "hx_search_dense_restricted_set_device",
 ]
 
 _lib = None
@@ -307,6 +308,12 @@ def load_library():
     L.hx_candidates_destroy.argtypes = [vp]
     L.hx_candidates_len.restype = C.c_uint64
     L.hx_candidates_len.argtypes = [vp]
+    L.hx_candidates_make_resident.restype = C.c_int32
+    L.hx_candidates_make_resident.argtypes = [vp, vp]
+    L.hx_candidates_resident_bytes.restype = C.c_uint64
+    L.hx_candidates_resident_bytes.argtypes = [vp]
+    L.hx_search_dense_restricted_set_device.restype = C.c_int32
+    L.hx_search_dense_restricted_set_device.argtypes = [vp, vp, sz, C.POINTER(_Params), vp, vp, vp, vp, vp, vp]
     L.hx_search_restricted_sets.restype = C.c_int32
     L.hx_search_restricted_sets.argtypes = [vp, fp, sz, C.POINTER(_Params), C.POINTER(vp), sz, u64p, fp, u32p,
                                             C.POINTER(SearchStats)]
@@ -524,11 +531,22 @@ class SearchParams:
 class DeviceCandidates:
     """A candidate set resident on the device (hx_candidates)."""
 
-    def __init__(self, L, h, n):
-        self.L, self.h, self.n = L, h, n
+    def __init__(self, L, h, n, ix=None):
+        self.L, self.h, self.n, self.ix = L, h, n, ix
 
     def __len__(self):
         return int(self.n)
+
+    def make_resident(self):
+        """hx_candidates_make_resident: build the set's tensor-core view once (blocking); the dense set entries then skip
+        the per-call compaction, gather and view reduction, and search_dense_restricted_set_device accepts the set."""
+        _ck(self.L.hx_candidates_make_resident(self.ix, self.h))
+        return self
+
+    @property
+    def resident_bytes(self):
+        """Device memory the resident view holds (0 while the set is not resident)."""
+        return int(self.L.hx_candidates_resident_bytes(self.h))
 
     def close(self):
         if self.h:
@@ -929,7 +947,7 @@ class VectorIndex:
         ca, cp = _u64(allowed.ids)
         h = C.c_void_p()
         _ck(self.L.hx_candidates_create(self.h, cp, ca.size, C.byref(h)))
-        return DeviceCandidates(self.L, h, ca.size)
+        return DeviceCandidates(self.L, h, ca.size, self.h)
 
     def search_restricted_sets(self, queries, params: SearchParams, sets, stats=None):
         """One DeviceCandidates per query, or a single one shared by all queries."""
@@ -1058,6 +1076,15 @@ class VectorIndex:
         _ck(self.L.hx_search_restricted_device(self.h, d_queries_ptr, B, C.byref(cp), d_slots_ptr, d_offsets_ptr,
                                                total, max_per_query, d_ids_ptr, d_scores_ptr, d_counts_ptr,
                                                stream_ptr))
+
+    def search_dense_restricted_set_device(self, d_queries_ptr, B, params: SearchParams, device_set: "DeviceCandidates",
+                                           d_ids_ptr, d_scores_ptr, d_counts_ptr, d_how_ptr=None, stream_ptr=0):
+        """hx_search_dense_restricted_set_device: the tensor-core path over a resident set (make_resident), enqueued on the
+        stream without synchronising.  d_how_ptr (B bytes, optional): 0 certified, 1 not certified (not rescanned), 2 exact
+        scan."""
+        cp = params._c()
+        _ck(self.L.hx_search_dense_restricted_set_device(self.h, d_queries_ptr, B, C.byref(cp), device_set.h, d_ids_ptr,
+                                                         d_scores_ptr, d_counts_ptr, d_how_ptr, stream_ptr))
 
     def map_candidates_device(self, d_ids_ptr, n, d_slots_ptr, stream_ptr=0):
         _ck(self.L.hx_map_candidates_device(self.h, d_ids_ptr, n, d_slots_ptr, None, stream_ptr))

@@ -444,6 +444,7 @@ static hx_status alloc_vectors(hx_index* ix, size_t n) {
   HX_CUDA(cudaMalloc((void**)&ix->d_ids, n * sizeof(uint64_t)));
   ix->n = n;
   ix->vector_generation++;
+  ix->content_epoch.fetch_add(1, std::memory_order_release);
   return HX_OK;
 }
 
@@ -2072,6 +2073,8 @@ struct hx_candidates {
   uint32_t* d_slots = nullptr;   // ascending; HX_ABSENT for ids without a vector row (never results)
   uint64_t n = 0;
   uint64_t generation = 0;
+  std::atomic<HxResident*> resident{nullptr};   // hx_candidates_make_resident: the tensor-core view, kept across calls
+  std::mutex resident_mu;                       // serialises the build; the view is published complete
 };
 
 extern "C" hx_status hx_candidates_create(hx_index* ix, const uint64_t* cand_ids, size_t n, hx_candidates** out) {
@@ -2116,14 +2119,41 @@ extern "C" hx_status hx_candidates_create(hx_index* ix, const uint64_t* cand_ids
 
 extern "C" void hx_candidates_destroy(hx_candidates* c) {
   if (!c) return;
-  if (c->d_slots) {
-    cudaSetDevice(c->ix->device);
-    cudaFree(c->d_slots);
-  }
+  if (c->d_slots || c->resident.load()) cudaSetDevice(c->ix->device);
+  if (c->d_slots) cudaFree(c->d_slots);
+  hx_resident_free(c->resident.load());
   delete c;
 }
 
 extern "C" uint64_t hx_candidates_len(const hx_candidates* c) { return c ? c->n : 0; }
+
+extern "C" hx_status hx_candidates_make_resident(hx_index* ix, hx_candidates* set) {
+  if (!ix || !set) {
+    hx_set_error("hx_candidates_make_resident: null argument");
+    return HX_ERR_INVALID_PARAMETER;
+  }
+  if (ix->cfg.metric == HX_METRIC_MANHATTAN) {
+    hx_set_error("the L1 metric is not a contraction: a candidate set of an L1 index has no tensor-core view");
+    return HX_ERR_UNSUPPORTED;
+  }
+  if (set->ix != ix || set->generation != ix->vector_generation) {
+    hx_set_error("candidate set does not belong to this index image (vectors were reloaded or deleted?)");
+    return HX_ERR_INVARIANT_VIOLATION;
+  }
+  std::lock_guard<std::mutex> lk(set->resident_mu);
+  if (set->resident.load()) return HX_OK;
+  HX_CUDA(cudaSetDevice(ix->device));
+  HxResident* r = nullptr;
+  hx_status rc = hx_resident_build(ix, set->d_slots, set->n, &r);
+  if (rc) return rc;
+  set->resident.store(r);
+  return HX_OK;
+}
+
+extern "C" uint64_t hx_candidates_resident_bytes(const hx_candidates* set) {
+  const HxResident* r = set ? set->resident.load() : nullptr;
+  return r ? r->bytes : 0;
+}
 
 extern "C" hx_status hx_search_restricted_sets(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
                                                hx_candidates* const* sets, size_t n_sets, uint64_t* out_ids,
@@ -2435,16 +2465,28 @@ static hx_status dense_restricted_host(hx_index* ix, const float* queries, size_
     launches++;
     slots = s->d_cand_slots.p;
   }
+  // a resident set (hx_candidates_make_resident) brings its present slots, tile and view word: no compaction (and no
+  // read-back of its count), no gather, no view reduction
+  HxResident* res = is_set ? set->resident.load() : nullptr;
   const uint32_t* d_present = nullptr;
   size_t present = 0;
-  if ((rc = hx_dense_compact(ix, s, slots, n, s->stream, &d_present, &present, &launches))) return rc;
+  if (res) {
+    if ((rc = hx_resident_current(ix, res))) return rc;
+    d_present = res->slots;
+    present = res->n;
+  } else if ((rc = hx_dense_compact(ix, s, slots, n, s->stream, &d_present, &present, &launches))) {
+    return rc;
+  }
   if ((rc = s->d_out_ids.reserve(B * (size_t)k)) || (rc = s->d_out_scores.reserve(B * (size_t)k)) ||
       (rc = s->d_out_counts.reserve(B)))
     return rc;
   // below the dense path's minimum the exact scan over the same slot list: hx_search_restricted's answer and launches
   const bool dense = present >= hx_dense_min_rows(k);
   HxDenseCert cert;
-  if (dense)
+  if (dense && res)
+    rc = hx_dense_resident_device(ix, s, s->d_queries.p, B, k, *res, s->d_out_ids.p, s->d_out_scores.p, s->d_out_counts.p,
+                                  s->stream, s->ev0, s->ev1, &launches, exact ? &cert : nullptr);
+  else if (dense)
     rc = hx_dense_restricted_device(ix, s, s->d_queries.p, B, k, d_present, present, s->d_out_ids.p, s->d_out_scores.p,
                                     s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches, exact ? &cert : nullptr);
   else
@@ -2479,8 +2521,9 @@ static hx_status dense_restricted_host(hx_index* ix, const float* queries, size_
     stats->kernel_launches = launches;
     if (dense) {
       stats->distance_computations = (uint64_t)B * present;
-      // gather (f32 rows in, bf16 tile and row terms out), then the tile read once by the contraction
-      stats->algorithmic_bytes = present * (4 * dim + 2 * ldb + 4) + present * 2 * ldb;
+      // gather (f32 rows in, bf16 tile and row terms out; none for a resident set), then the tile read once by the
+      // contraction
+      stats->algorithmic_bytes = (res ? 0 : present * (4 * dim + 2 * ldb + 4)) + present * 2 * ldb;
       stats->reserved = (uint64_t)(2.0 * (double)B * (double)present * (double)ldb);   // flop of the contraction
       if (flagged) {   // the rescanned queries' full scans over the present rows
         stats->distance_computations += flagged * present;
@@ -2522,6 +2565,76 @@ extern "C" hx_status hx_search_dense_restricted_exact_set(hx_index* ix, const fl
                                                           uint8_t* out_how, hx_stats* stats) {
   return dense_restricted_host(ix, queries, B, p, nullptr, 0, set, true, out_ids, out_scores, out_counts, stats, true,
                                out_how);
+}
+
+// hx_search_dense_restricted_set on device buffers, through a resident set: everything on the caller's stream, no
+// synchronisation once the view is current.  Admission is hx_search_dense_restricted_set's, in its order, then the set
+// must be resident.  d_out_how (may be null): the certificate without the rescan (0 certified, 1 not certified), or 2
+// for every query when the present rows are below hx_dense_min_rows(k) and the exact scan answered.
+extern "C" hx_status hx_search_dense_restricted_set_device(hx_index* ix, const float* d_queries, size_t B,
+                                                           const hx_search_params* p, const hx_candidates* set,
+                                                           uint64_t* d_out_ids, float* d_out_scores, uint32_t* d_out_counts,
+                                                           uint8_t* d_out_how, void* cuda_stream) {
+  if (!ix) {
+    hx_set_error("null index handle");
+    return HX_ERR_INDEX_NOT_FOUND;
+  }
+  uint32_t k, ef;
+  hx_status rc = check_params(ix, p, &k, &ef);
+  if (rc) return rc;
+  if (B == 0) return HX_OK;
+  if (!d_queries || !d_out_ids || !d_out_scores || !d_out_counts || !set) return HX_ERR_INVALID_PARAMETER;
+  if (ix->cfg.metric == HX_METRIC_MANHATTAN) {
+    hx_set_error("the L1 metric is not a contraction: use hx_search_restricted_device");
+    return HX_ERR_UNSUPPORTED;
+  }
+  cudaStream_t stream = (cudaStream_t)cuda_stream;
+  auto answer_none = [&]() -> hx_status {   // counts 0, every query "answered by the exact scan"
+    HX_CUDA(cudaSetDevice(ix->device));
+    HX_CUDA(cudaMemsetAsync(d_out_counts, 0, B * sizeof(uint32_t), stream));
+    if (d_out_how) HX_CUDA(cudaMemsetAsync(d_out_how, 2, B, stream));
+    return HX_OK;
+  };
+  const uint64_t n = set->n;
+  if (n > 1000000ull) {
+    hx_set_error("restricted vector search accepts at most 1000000 unique candidates");
+    return HX_ERR_QUERY;
+  }
+  if (n == 0) return answer_none();
+  if (std::min<uint64_t>(k, n) > 800) {
+    hx_set_error("restricted vector search result count must be at most 800, got %llu",
+                 (unsigned long long)std::min<uint64_t>(k, n));
+    return HX_ERR_QUERY;
+  }
+  if (set->ix != ix || set->generation != ix->vector_generation) {
+    hx_set_error("candidate set does not belong to this index image (vectors were reloaded or deleted?)");
+    return HX_ERR_INVARIANT_VIOLATION;
+  }
+  HxResident* res = set->resident.load();
+  if (!res) {
+    hx_set_error("hx_search_dense_restricted_set_device needs a resident set (hx_candidates_make_resident)");
+    return HX_ERR_INVALID_PARAMETER;
+  }
+  HX_CUDA(cudaSetDevice(ix->device));
+  if (ix->n == 0 || !ix->populated || res->n == 0) return answer_none();
+  if ((rc = hx_resident_current(ix, res))) return rc;
+  HxScratch* s = nullptr;
+  if ((rc = dev_scratch(ix, stream, &s))) return rc;
+  uint32_t launches = 0;
+  if ((rc = prepare_device_queries(ix, s, d_queries, B, stream, &launches))) return rc;
+  cudaEvent_t e0, e1;
+  if ((rc = s->ring_next(&e0, &e1))) return rc;
+  if (res->n < hx_dense_min_rows(k)) {   // the exact scan over the present slots
+    if (d_out_how) HX_CUDA(cudaMemsetAsync(d_out_how, 2, B, stream));
+    return launch_scan_select(ix, s, d_queries, B, k, res->slots, nullptr, true, res->n, res->n, (uint64_t)B * res->n,
+                              d_out_ids, d_out_scores, d_out_counts, stream, e0, e1, &launches);
+  }
+  HxDenseCert cert;
+  if ((rc = hx_dense_resident_device(ix, s, d_queries, B, k, *res, d_out_ids, d_out_scores, d_out_counts, stream, e0, e1,
+                                     &launches, d_out_how ? &cert : nullptr)))
+    return rc;
+  if (d_out_how) HX_CUDA(cudaMemcpyAsync(d_out_how, cert.how, B, cudaMemcpyDeviceToDevice, stream));
+  return HX_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -197,6 +197,9 @@ struct hx_index {
   size_t n_live = 0;
   void* d_vec_bf16 = nullptr;
   float* d_sqnorm = nullptr;
+  // row contents: bumped wherever the whole-corpus bf16 copy is dropped and wherever vector_generation moves, so a resident
+  // candidate view (HxResident) knows that its gathered tile no longer holds the rows' current values
+  std::atomic<uint64_t> content_epoch{0};
   // scratch pool
   std::mutex mu;
   std::condition_variable cv;
@@ -268,3 +271,29 @@ hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* 
                                      const uint32_t* d_present, size_t n_present, uint64_t* d_out_ids, float* d_out_sc,
                                      uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1,
                                      uint32_t* launches, HxDenseCert* cert = nullptr);
+
+// The resident tensor-core view of a device candidate set (hx_candidates_make_resident): what
+// hx_search_dense_restricted_set otherwise rebuilds on every call, built once and kept by the set.  The present list never
+// changes while the set is valid (deletes and reloads move vector_generation, which refuses the set; upserts do not touch
+// the set's slots), so only the row values can go stale: `epoch` is the index's content_epoch the tile was gathered at.
+struct HxResident {
+  std::mutex mu;                     // held by a refresh; a new epoch is published under it once the tile is complete
+  std::atomic<uint64_t> epoch{0};
+  cudaStream_t stream = nullptr;     // builds and refreshes run here, never on a caller's stream
+  uint32_t* slots = nullptr;         // [n] the set's present slots, ascending (hx_dense_compact)
+  size_t n = 0;
+  void* rows = nullptr;              // [n rounded up to 256][ldb] bf16, tile placement over candidate rank (k_to_bf16)
+  float* aux = nullptr;              // row terms by position, then (at the end) k_dense_view_bound's word
+  uint32_t* word = nullptr;
+  uint64_t bytes = 0;                // device memory held
+};
+// hx_candidates_make_resident: compaction of the set's slot list, gather, view word; blocking.  *out is set on success.
+hx_status hx_resident_build(hx_index* ix, const uint32_t* d_slots, size_t n_slots, HxResident** out);
+// the first call after a row write re-gathers the tile and the view word in place (same present list); otherwise nothing
+hx_status hx_resident_current(hx_index* ix, HxResident* r);
+void hx_resident_free(HxResident* r);
+// hx_dense_restricted_device over a resident view (r.n >= hx_dense_min_rows(k)): no compaction, no gather, and the
+// certificate reads the view word the view holds
+hx_status hx_dense_resident_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxResident& r,
+                                   uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
+                                   cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches, HxDenseCert* cert = nullptr);

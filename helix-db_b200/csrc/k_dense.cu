@@ -928,23 +928,33 @@ static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size
   return HX_OK;
 }
 
+// k_dense_view_bound over view `v` into *word (zeroed first), enqueued on `stream`
+static hx_status dense_view_word(hx_index* ix, const HxDenseView& v, uint32_t* word, cudaStream_t stream) {
+  HX_CUDA(cudaMemsetAsync(word, 0, 4, stream));
+  const size_t n_pad = (v.n + HXD_BN - 1) / HXD_BN * HXD_BN;
+  const unsigned grid = (unsigned)std::min<size_t>((n_pad + 255) / 256, 4 * (size_t)std::max(1, ix->sm_count));
+  k_dense_view_bound<<<grid, 256, 0, stream>>>(v.aux, ix->d_hdr, v.slots, v.n, ix->cfg.metric, word);
+  HX_CUDA(cudaGetLastError());
+  return HX_OK;
+}
+
 // The certificate after a pass over view `v` (see k_dense_certify), then the order-preserving compaction of the flagged
 // query indices.  Enqueued on `stream`, no synchronisation.  Buffers: the scratch set's x_flag / x_how, none of the pass's.
+// `resident_word`: the view's word as a resident view holds it (null: reduced here, one more launch).
 static hx_status dense_certify(hx_index* ix, HxScratch* scr, size_t B, uint32_t k, const HxDenseView& v,
                                const HxDensePassOut& po, const float* d_out_sc, const uint32_t* d_out_cnt, HxDenseCert* cert,
-                               cudaStream_t stream, uint32_t* launches) {
+                               cudaStream_t stream, uint32_t* launches, const uint32_t* resident_word = nullptr) {
   hx_status rc;
   const size_t tiles = (B + HXD_CPT_TILE - 1) / HXD_CPT_TILE;
   if ((rc = scr->x_flag.reserve(2 * B + tiles + 2)) || (rc = scr->x_how.reserve(B))) return rc;
   uint32_t* flag = scr->x_flag.p;          // [B] per query
   uint32_t* flagged = flag + B;            // [B] compacted
   uint32_t* counts = flagged + B;          // [tiles] + the total
-  uint32_t* view_word = counts + tiles + 1;   // k_dense_view_bound
-  {
-    HX_CUDA(cudaMemsetAsync(view_word, 0, 4, stream));
-    const size_t n_pad = (v.n + HXD_BN - 1) / HXD_BN * HXD_BN;
-    const unsigned grid = (unsigned)std::min<size_t>((n_pad + 255) / 256, 4 * (size_t)std::max(1, ix->sm_count));
-    k_dense_view_bound<<<grid, 256, 0, stream>>>(v.aux, ix->d_hdr, v.slots, v.n, ix->cfg.metric, view_word);
+  const uint32_t* view_word = resident_word;
+  if (!view_word) {
+    uint32_t* w = counts + tiles + 1;
+    if ((rc = dense_view_word(ix, v, w, stream))) return rc;
+    view_word = w;
     ++*launches;
   }
   HxCertArgs a{};
@@ -1035,6 +1045,23 @@ hx_status hx_dense_compact(hx_index* ix, HxScratch* scr, const uint32_t* d_slots
   return HX_OK;
 }
 
+// The tensor-core pass over a candidate view, then (cert != null) the certificate; `view_word` as dense_certify's
+// resident_word.  Adds the launches it issues to *launches.
+static hx_status dense_view_search(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxDenseView& v,
+                                   const uint32_t* view_word, uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt,
+                                   cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches,
+                                   HxDenseCert* cert) {
+  hx_status rc;
+  uint32_t pass_launches = 0;
+  HxDensePassOut po{};
+  if ((rc = dense_pass(ix, scr, d_q, B, k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, &pass_launches,
+                       cert ? &po : nullptr)))
+    return rc;
+  *launches += pass_launches;
+  if (cert) return dense_certify(ix, scr, B, k, v, po, d_out_sc, d_out_cnt, cert, stream, launches, view_word);
+  return HX_OK;
+}
+
 // hx_search_dense_restricted, step 2 (n_present >= hx_dense_min_rows(k)): the present rows, converted from the f32 rows into
 // a bf16 tile of this scratch set's own (k_to_bf16: tile placement over candidate RANK, cosine power-of-two scaling, row
 // terms), then the tensor-core pass over that tile with the compacted slots as its slot table.  The whole-corpus bf16 copy
@@ -1055,15 +1082,91 @@ hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* 
   k_to_bf16<<<(unsigned)((n_present + 7) / 8), 256, 0, stream>>>(ix->d_vec, n_present, ix->cfg.dimension, ix->ld,
                                                                  (__nv_bfloat16*)tile, ldb, aux, ix->cfg.metric, 1, d_present);
   HX_CUDA(cudaGetLastError());
-  const HxDenseView v{tile, aux, d_present, n_present};
-  uint32_t pass_launches = 0;
-  HxDensePassOut po{};
-  if ((rc = dense_pass(ix, scr, d_q, B, k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, &pass_launches,
-                       cert ? &po : nullptr)))
-    return rc;
-  *launches += 1 + pass_launches;
-  if (cert) return dense_certify(ix, scr, B, k, v, po, d_out_sc, d_out_cnt, cert, stream, launches);
+  *launches += 1;
+  return dense_view_search(ix, scr, d_q, B, k, HxDenseView{tile, aux, d_present, n_present}, nullptr, d_out_ids, d_out_sc,
+                           d_out_cnt, stream, e0, e1, launches, cert);
+}
+
+// ---- resident candidate views (hx_candidates_make_resident) -------------------------------------------------------------------
+// The tile, its row terms and the view word of a resident view, from the current f32 rows of its present slots: the same
+// kernels, on the same rows, as hx_dense_restricted_device and dense_certify run per call, so a search through the view
+// returns the non-resident set's answer bit for bit.  Enqueued on r->stream, then ONE synchronisation.
+static hx_status resident_fill(hx_index* ix, HxResident* r) {
+  const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
+  k_to_bf16<<<(unsigned)((r->n + 7) / 8), 256, 0, r->stream>>>(ix->d_vec, r->n, ix->cfg.dimension, ix->ld,
+                                                                (__nv_bfloat16*)r->rows, ldb, r->aux, ix->cfg.metric, 1,
+                                                                r->slots);
+  HX_CUDA(cudaGetLastError());
+  hx_status rc = dense_view_word(ix, HxDenseView{r->rows, r->aux, r->slots, r->n}, r->word, r->stream);
+  if (rc) return rc;
+  HX_CUDA(cudaStreamSynchronize(r->stream));
   return HX_OK;
+}
+
+void hx_resident_free(HxResident* r) {
+  if (!r) return;
+  if (r->stream) cudaStreamDestroy(r->stream);
+  if (r->slots) cudaFree(r->slots);
+  if (r->rows) cudaFree(r->rows);
+  if (r->aux) cudaFree(r->aux);
+  delete r;
+}
+
+hx_status hx_resident_build(hx_index* ix, const uint32_t* d_slots, size_t n_slots, HxResident** out) {
+  HxResident* r = new HxResident();
+  struct Free { HxResident*& r; ~Free() { hx_resident_free(r); } } fr{r};   // unless published below
+  const uint64_t epoch = ix->content_epoch.load(std::memory_order_acquire);
+  HX_CUDA(cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking));
+  if (n_slots) {
+    HxScratch* s = nullptr;
+    hx_status rc = hx_acquire_scratch(ix, &s);
+    if (rc) return rc;
+    struct Rel { hx_index* ix; HxScratch* s; ~Rel() { hx_release_scratch(ix, s); } } rel{ix, s};
+    const uint32_t* d_present = nullptr;
+    uint32_t launches = 0;
+    if ((rc = hx_dense_compact(ix, s, d_slots, n_slots, r->stream, &d_present, &r->n, &launches))) return rc;
+    if (r->n) {
+      const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
+      const size_t n_pad = (r->n + HXD_BN - 1) / HXD_BN * HXD_BN;
+      HX_CUDA(cudaMalloc((void**)&r->slots, r->n * 4));
+      HX_CUDA(cudaMalloc(&r->rows, n_pad * (size_t)ldb * 2));
+      HX_CUDA(cudaMalloc((void**)&r->aux, (n_pad + 1) * 4));
+      r->word = reinterpret_cast<uint32_t*>(r->aux + n_pad);
+      r->bytes = n_pad * (uint64_t)(2 * ldb + 4) + 4 * (uint64_t)r->n + 4;
+      HX_CUDA(cudaMemcpyAsync(r->slots, d_present, r->n * 4, cudaMemcpyDeviceToDevice, r->stream));
+      // the positions of the last placement tile that no candidate fills read as zero rows, for good: refreshes rewrite
+      // the present positions only
+      HX_CUDA(cudaMemsetAsync(r->rows, 0, n_pad * (size_t)ldb * 2, r->stream));
+      HX_CUDA(cudaMemsetAsync(r->aux, 0, n_pad * 4, r->stream));
+      if ((rc = resident_fill(ix, r))) return rc;
+    }
+  }
+  r->epoch.store(epoch, std::memory_order_release);
+  *out = r;
+  r = nullptr;
+  return HX_OK;
+}
+
+// The pattern of ensure_dense_state: a caller that finds the view stale takes the view's mutex, re-checks, re-gathers on the
+// view's own stream, synchronises once and only then publishes the epoch; concurrent first callers wait on the mutex and
+// find it current, so the tile is rebuilt once and never read half built.  In place: a stream-ordered search that still
+// reads the tile counts as overlapping the row write that made it stale (patch calls must not overlap searches).
+hx_status hx_resident_current(hx_index* ix, HxResident* r) {
+  const uint64_t want = ix->content_epoch.load(std::memory_order_acquire);
+  if (r->n == 0 || r->epoch.load(std::memory_order_acquire) == want) return HX_OK;
+  std::lock_guard<std::mutex> lk(r->mu);
+  if (r->epoch.load(std::memory_order_acquire) == want) return HX_OK;
+  hx_status rc = resident_fill(ix, r);
+  if (rc) return rc;
+  r->epoch.store(want, std::memory_order_release);
+  return HX_OK;
+}
+
+hx_status hx_dense_resident_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxResident& r,
+                                   uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
+                                   cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches, HxDenseCert* cert) {
+  return dense_view_search(ix, scr, d_q, B, k, HxDenseView{r.rows, r.aux, r.slots, r.n}, r.word, d_out_ids, d_out_sc,
+                           d_out_cnt, stream, e0, e1, launches, cert);
 }
 
 // Host-buffer entry point: a private stream + scratch set per call, the queries cross PCIe with one async copy, results

@@ -197,6 +197,10 @@ class VectorIndex {
     for (uint32_t i = 0; i < count; ++i) out[i] = SearchResult{ids[i], scores[i]};
     return out;
   }
+  // A device candidate set's tensor-core view, built once and kept by the set (hx_candidates_make_resident), and the
+  // device memory it holds (0 while the set is not resident)
+  void make_resident(hx_candidates* set) const { check(hx_candidates_make_resident(h_, set)); }
+  static uint64_t resident_bytes(const hx_candidates* set) { return hx_candidates_resident_bytes(set); }
   hx_index* raw() const { return h_; }
   uint32_t dimension() const { return dim_; }
 

@@ -550,6 +550,47 @@ hx_status hx_search_dense_restricted_exact_set(hx_index* idx, const float* queri
                                                const hx_candidates* set, uint64_t* out_ids, float* out_scores,
                                                uint32_t* out_counts, uint8_t* out_how, hx_stats* stats);
 
+/* Resident candidate sets.  hx_search_dense_restricted_set and _exact_set otherwise rebuild the set's tensor-core view on
+ * every call: compaction of the present slots (and a stream synchronisation to read their count), gather of the present
+ * rows into a bf16 tile, and for the exact entry the reduction of the view word of the certificate.  The gather is the
+ * largest kernel of a call.  hx_candidates_make_resident builds that view once, blocking, and the set keeps it until
+ * hx_candidates_destroy.  It holds the ascending present slots, the bf16 tile in tile placement over candidate rank, the
+ * row terms and the view word, built by the kernels the per-call path runs, so an answer through a resident set is the
+ * answer of the same ids through a non-resident set bit for bit.
+ * With the view, the two set entries run no compaction, gather or view reduction: the plain entry synchronises once per call.
+ * hx_stats: kernel_launches counts the launches actually issued; algorithmic_bytes = present * 2 * ldb (the tile read once)
+ * plus any rescans.
+ * Device memory: n_pad * (2 * ldb + 4) + 4 * present + 4 bytes (n_pad = present rounded up to 256, ldb = the dimension
+ * rounded up to 64; 0 when no id of the set is present), about 1.5 GB at present = 1e6, d = 768.  hx_candidates_resident_bytes
+ * reports it (0 while the set is not resident).
+ * Admission, in order: null argument => HX_ERR_INVALID_PARAMETER; Manhattan => HX_ERR_UNSUPPORTED; a set of another index or
+ * of an older vector generation => HX_ERR_INVARIANT_VIOLATION; an empty set => HX_OK, 0 bytes.  A second call is a no-op.
+ * Staleness: the present list cannot change while the set is valid (deletes and reloads refuse the set; upserts do not
+ * remap it), but an upsert can change row values.  The first call after any row write re-gathers the tile and the view word
+ * in place, on the set's own stream, once, however many callers race to it; no caller reads a half-built tile.  A
+ * stream-ordered search (hx_search_dense_restricted_set_device) counts as overlapping a patch call until its stream has
+ * been synchronised: patch calls must not overlap searches, and a patch must not run while such a search may still read
+ * the tile.  A set maps its ids once, at hx_candidates_create: ids appended or revived by later upserts stay absent from
+ * it, resident or not. */
+hx_status hx_candidates_make_resident(hx_index* idx, hx_candidates* set);
+uint64_t  hx_candidates_resident_bytes(const hx_candidates* set);
+/* hx_search_dense_restricted_set on device buffers, through a resident set.  Everything is enqueued on `cuda_stream`
+ * (per-stream scratch, as hx_search_device); no synchronisation once the view is current (the first call after a row
+ * write refreshes it as above).  Admission exactly as hx_search_dense_restricted_set, in its order; then a set that is not
+ * resident => HX_ERR_INVALID_PARAMETER.  d_queries follow hx_search_device's convention: the caller validates them, an
+ * invalid query gets count 0.  Device errors come out through hx_device_flags.  Below hx_dense_min_rows(k) present rows
+ * the exact scan over the present slots answers, on the stream.
+ * d_out_how (B bytes on the device, may be NULL) runs the certificate of the exact entries without the rescan:
+ *   0 = certified: the answer is hx_search_restricted's bit for bit;
+ *   1 = not certified: the plain tensor-core answer is returned, not rescanned;
+ *   2 = the present rows are below hx_dense_min_rows(k): exact scan.
+ * The rescan needs the flagged count on the host, so a caller that needs exactness for the queries marked 1 re-issues them
+ * through hx_search_restricted_device or an exact host entry. */
+hx_status hx_search_dense_restricted_set_device(hx_index* idx, const float* d_queries, size_t B, const hx_search_params* p,
+                                                const hx_candidates* set, uint64_t* d_out_ids, float* d_out_scores,
+                                                uint32_t* d_out_counts, uint8_t* d_out_how /* may be NULL */,
+                                                void* cuda_stream);
+
 /* ---- SimHash filtering / sampling policy: the production-default search mode ------------------------------
  * SearchParams::new(k) is SimHashMode::Adaptive: layer 0 then runs Layer0Policy::decide per expansion
  * (policy.rs:119-175: adaptive collision threshold :576-597, adaptive sampling :558-574, pre-/post-sampling activation
