@@ -22,11 +22,16 @@ class CallersReport(C.Structure):
 def load():
     global _LIB
     if _LIB is None:
-        from . import load_library
+        from . import LIB_PATH, load_library
         load_library()   # libhelix_b200.so first (the harness links against it)
         p = Path(__file__).resolve().parent / "libhx_callers.so"
         if not p.exists():
             raise RuntimeError(f"{p} is missing: run helix-db_b200/build.sh")
+        # The harness must call the library this process already loaded, which HELIX_B200_LIB may have taken from
+        # another build.  Its link-time dependency is the copy beside it; promoting the loaded library to the global
+        # scope binds the harness's hx_* symbols to the loaded one instead.  Otherwise the two builds would share
+        # handles, and each would read the other's structures.
+        C.CDLL(str(LIB_PATH), mode=C.RTLD_GLOBAL)
         L = C.CDLL(str(p))
         L.hx_callers_run.restype = C.c_int
         L.hx_callers_run.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.c_float), C.c_size_t, C.c_uint32,

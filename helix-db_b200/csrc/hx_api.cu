@@ -236,9 +236,7 @@ void HxScratch::destroy() {
   d_tiepool.release(); d_tiebusy.release(); d_qerr.release(); h_qerr.release(); d_partial.release(); d_tickets.release();
   d_fg_stamps.release(); d_fg_epochs.release(); d_fg_bridge.release(); d_fg_elig.release(); d_fg_bits.release(); d_fg_seed.release();
   d_vtab.release(); d_vpool.release(); d_vbusy.release(); d_prof.release(); d_pstats.release(); d_qsim.release();
-  for (auto& m : misc) m.release();
-  x_flag.release(); x_status.release(); x_counts.release(); x_how.release(); x_queries.release(); x_hdr.release();
-  x_scores.release(); x_ids.release(); h_x.release();
+  dense.release();
   h_ids.release(); h_cand_offsets.release(); h_scores.release(); h_queries.release(); h_qhdr.release();
   h_counts.release(); h_qstats.release(); h_status.release(); h_err.release(); h_avail.release();
   d_block.release(); h_block.release();
@@ -1943,6 +1941,30 @@ static hx_status launch_scan_select(hx_index* ix, HxScratch* s, const float* d_q
   return HX_OK;
 }
 
+// The download of an exact-scan-style answer from s->d_out_* (ids, scores, counts, per-query status words, the device error
+// word) with ONE synchronisation of s->stream, then the report: the first query that failed validation, the device flags
+// (or-ed with `flags_before`, what an earlier scan of the call left), and the timing of the scan's events.
+static hx_status download_report(hx_index* ix, HxScratch* s, size_t B, uint32_t k, uint64_t* out_ids, float* out_scores,
+                                 uint32_t* out_counts, uint32_t flags_before = 0) {
+  hx_status rc;
+  if ((rc = s->h_status.reserve(B)) || (rc = s->h_err.reserve(1))) return rc;
+  HX_CUDA(cudaMemcpyAsync(out_ids, s->d_out_ids.p, B * (size_t)k * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaMemcpyAsync(out_scores, s->d_out_scores.p, B * (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaMemcpyAsync(out_counts, s->d_out_counts.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaMemcpyAsync(s->h_status.p, s->d_qstatus.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaMemcpyAsync(s->h_err.p, s->d_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
+  HX_CUDA(cudaStreamSynchronize(s->stream));
+  for (size_t b = 0; b < B; ++b)
+    if (s->h_status.p[b] != HX_ST_OK) return status_from_word(s->h_status.p[b], b, "query");
+  if ((rc = check_device_flags(s->h_err.p[0] | flags_before))) return rc;
+  float ms = 0.f;
+  if (cudaEventElapsedTime(&ms, s->ev0, s->ev1) == cudaSuccess) {
+    ix->last_kernel_ms = ms;
+    ix->last_kernel_launches = 1;
+  }
+  return HX_OK;
+}
+
 static hx_status restricted_host(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
                                  const uint64_t* cand_ids, const uint64_t* cand_offsets, size_t n_shared, bool shared,
                                  uint64_t* out_ids, float* out_scores, uint32_t* out_counts, hx_stats* stats) {
@@ -2023,24 +2045,9 @@ static hx_status restricted_host(hx_index* ix, const float* queries, size_t B, c
   const uint64_t total_keys = shared ? (uint64_t)B * n_shared : total;
   if ((rc = launch_scan_select(ix, s, s->d_queries.p, B, k, s->d_cand_slots.p, s->d_cand_offsets.p, shared, n_shared,
                                max_c, total_keys, s->d_out_ids.p, s->d_out_scores.p, s->d_out_counts.p, s->stream,
-                               s->ev0, s->ev1, &launches)))
+                               s->ev0, s->ev1, &launches)) ||
+      (rc = download_report(ix, s, B, k, out_ids, out_scores, out_counts)))
     return rc;
-  if ((rc = s->h_status.reserve(B))) return rc;
-  if ((rc = s->h_err.reserve(1))) return rc;
-  HX_CUDA(cudaMemcpyAsync(out_ids, s->d_out_ids.p, B * (size_t)k * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(out_scores, s->d_out_scores.p, B * (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(out_counts, s->d_out_counts.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(s->h_status.p, s->d_qstatus.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(s->h_err.p, s->d_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaStreamSynchronize(s->stream));
-  for (size_t b = 0; b < B; ++b)
-    if (s->h_status.p[b] != HX_ST_OK) return status_from_word(s->h_status.p[b], b, "query");
-  if ((rc = check_device_flags(s->h_err.p[0]))) return rc;
-  float ms = 0.f;
-  if (cudaEventElapsedTime(&ms, s->ev0, s->ev1) == cudaSuccess) {
-    ix->last_kernel_ms = ms;
-    ix->last_kernel_launches = 1;
-  }
   if (stats) {
     stats->kernel_launches = launches;
     stats->distance_computations = total_keys;
@@ -2218,24 +2225,9 @@ extern "C" hx_status hx_search_restricted_sets(hx_index* ix, const float* querie
   if ((rc = s->d_out_scores.reserve(B * (size_t)k))) return rc;
   if ((rc = s->d_out_counts.reserve(B))) return rc;
   if ((rc = launch_scan_select(ix, s, s->d_queries.p, B, k, nullptr, nullptr, false, 0, max_c, total_keys, s->d_out_ids.p,
-                               s->d_out_scores.p, s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches, &refs)))
+                               s->d_out_scores.p, s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches, &refs)) ||
+      (rc = download_report(ix, s, B, k, out_ids, out_scores, out_counts)))
     return rc;
-  if ((rc = s->h_status.reserve(B))) return rc;
-  if ((rc = s->h_err.reserve(1))) return rc;
-  HX_CUDA(cudaMemcpyAsync(out_ids, s->d_out_ids.p, B * (size_t)k * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(out_scores, s->d_out_scores.p, B * (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(out_counts, s->d_out_counts.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(s->h_status.p, s->d_qstatus.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(s->h_err.p, s->d_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaStreamSynchronize(s->stream));
-  for (size_t b = 0; b < B; ++b)
-    if (s->h_status.p[b] != HX_ST_OK) return status_from_word(s->h_status.p[b], b, "query");
-  if ((rc = check_device_flags(s->h_err.p[0]))) return rc;
-  float ms = 0.f;
-  if (cudaEventElapsedTime(&ms, s->ev0, s->ev1) == cudaSuccess) {
-    ix->last_kernel_ms = ms;
-    ix->last_kernel_launches = 1;
-  }
   if (stats) {
     stats->kernel_launches = launches;
     stats->distance_computations = total_keys;
@@ -2317,325 +2309,7 @@ extern "C" hx_status hx_merge_topk_device(int32_t device, const uint64_t* d_all_
   return HX_OK;
 }
 
-extern "C" hx_status hx_search_dense(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
-                                     uint64_t* out_ids, float* out_scores, uint32_t* out_counts, hx_stats* stats) {
-  if (!ix) return HX_ERR_INDEX_NOT_FOUND;
-  HX_CUDA(cudaSetDevice(ix->device));
-  return hx_dense_impl(ix, queries, B, p, out_ids, out_scores, out_counts, stats);
-}
-
-extern "C" hx_status hx_search_dense_exact(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
-                                           uint64_t* out_ids, float* out_scores, uint32_t* out_counts, uint8_t* out_how,
-                                           hx_stats* stats) {
-  if (!ix) return HX_ERR_INDEX_NOT_FOUND;
-  HX_CUDA(cudaSetDevice(ix->device));
-  return hx_dense_impl(ix, queries, B, p, out_ids, out_scores, out_counts, stats, true, out_how);
-}
-
-// rescan, step 1: flagged query j (query flagged[j] of the call) -> row j of a contiguous batch, with its header and status
-// word.  One warp per flagged query.
-static __global__ void k_dense_gather(const float* __restrict__ q, const float* __restrict__ hdr,
-                                      const uint32_t* __restrict__ status, const uint32_t* __restrict__ flagged, size_t F,
-                                      uint32_t dim, float* __restrict__ gq, float* __restrict__ ghdr,
-                                      uint32_t* __restrict__ gstatus) {
-  const size_t j = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t lane = threadIdx.x & 31u;
-  if (j >= F) return;
-  const size_t b = flagged[j];
-  for (uint32_t i = lane; i < dim; i += 32) gq[j * dim + i] = q[b * dim + i];
-  if (lane == 0) {
-    ghdr[j] = hdr[b];
-    gstatus[j] = status[b];
-  }
-}
-
-// rescan, step 3: the exact answer of flagged query j replaces the output row of query flagged[j]
-static __global__ void k_dense_scatter(const uint64_t* __restrict__ gids, const float* __restrict__ gsc,
-                                       const uint32_t* __restrict__ gcnt, const uint32_t* __restrict__ flagged, size_t F,
-                                       uint32_t k, uint64_t* __restrict__ ids, float* __restrict__ sc, uint32_t* __restrict__ cnt) {
-  const size_t j = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t lane = threadIdx.x & 31u;
-  if (j >= F) return;
-  const size_t b = flagged[j];
-  const uint32_t c = gcnt[j];
-  for (uint32_t i = lane; i < c; i += 32) {
-    ids[b * k + i] = gids[j * k + i];
-    sc[b * k + i] = gsc[j * k + i];
-  }
-  if (lane == 0) cnt[b] = c;
-}
-
-hx_status hx_dense_rescan(hx_index* ix, HxScratch* s, const float* d_q, uint32_t k, const uint32_t* slots,
-                          size_t n_view, const HxDenseCert& cert, uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt,
-                          cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches, size_t* n_flagged,
-                          uint32_t* err_before) {
-  hx_status rc;
-  if ((rc = s->h_x.reserve(2)) || (rc = s->d_err.reserve(1))) return rc;
-  HX_CUDA(cudaMemcpyAsync(s->h_x.p, cert.n_flagged, 4, cudaMemcpyDeviceToHost, stream));
-  HX_CUDA(cudaMemcpyAsync(s->h_x.p + 1, s->d_err.p, 4, cudaMemcpyDeviceToHost, stream));
-  HX_CUDA(cudaStreamSynchronize(stream));
-  const size_t F = s->h_x.p[0];
-  *n_flagged = F;
-  *err_before = s->h_x.p[1];
-  if (F == 0) return HX_OK;
-  const uint32_t dim = ix->cfg.dimension;
-  if ((rc = s->x_queries.reserve(F * (size_t)dim)) || (rc = s->x_hdr.reserve(F)) || (rc = s->x_status.reserve(F)) ||
-      (rc = s->x_ids.reserve(F * (size_t)k)) || (rc = s->x_scores.reserve(F * (size_t)k)) || (rc = s->x_counts.reserve(F)))
-    return rc;
-  const unsigned grid = (unsigned)((F + 7) / 8);
-  k_dense_gather<<<grid, 256, 0, stream>>>(d_q, s->d_qhdr.p, s->d_qstatus.p, cert.flagged, F, dim, s->x_queries.p,
-                                           s->x_hdr.p, s->x_status.p);
-  HX_CUDA(cudaGetLastError());
-  ++*launches;
-  if ((rc = launch_scan_select(ix, s, s->x_queries.p, F, k, slots, nullptr, true, n_view, n_view, (uint64_t)F * n_view,
-                               s->x_ids.p, s->x_scores.p, s->x_counts.p, stream, e0, e1, launches, nullptr, s->x_hdr.p,
-                               s->x_status.p)))
-    return rc;
-  k_dense_scatter<<<grid, 256, 0, stream>>>(s->x_ids.p, s->x_scores.p, s->x_counts.p, cert.flagged, F, k, d_out_ids, d_out_sc,
-                                            d_out_cnt);
-  HX_CUDA(cudaGetLastError());
-  ++*launches;
-  return HX_OK;
-}
-
-// The dense path over one candidate set shared by the B queries: host ids (`cand_ids`, n_cand) or a device set (`set`).
-// Admission is restricted_host's, in its order, with the dense path's metric check before anything about the set.
-// `exact` (hx_search_dense_restricted_exact[_set]): the certificate follows the re-rank and the queries it cannot clear are
-// rescanned over the present slots; out_how (may be null) as hx_search_dense_exact's.
-static hx_status dense_restricted_host(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
-                                       const uint64_t* cand_ids, size_t n_cand, const hx_candidates* set, bool is_set,
-                                       uint64_t* out_ids, float* out_scores, uint32_t* out_counts, hx_stats* stats,
-                                       bool exact = false, uint8_t* out_how = nullptr) {
-  if (!ix) {
-    hx_set_error("null index handle");
-    return HX_ERR_INDEX_NOT_FOUND;
-  }
-  uint32_t k, ef;
-  hx_status rc = check_params(ix, p, &k, &ef);
-  if (rc) return rc;
-  if (stats) memset(stats, 0, sizeof(*stats));
-  if (B == 0) return HX_OK;
-  if (!queries || !out_ids || !out_scores || !out_counts || (is_set ? !set : (n_cand && !cand_ids))) return HX_ERR_INVALID_PARAMETER;
-  if (ix->cfg.metric == HX_METRIC_MANHATTAN) {
-    hx_set_error("the L1 metric is not a contraction: use hx_search_restricted");
-    return HX_ERR_UNSUPPORTED;
-  }
-  if (exact && out_how) memset(out_how, 2, B);
-  const uint64_t n = is_set ? set->n : n_cand;
-  if (n > 1000000ull) {
-    hx_set_error("restricted vector search accepts at most 1000000 unique candidates");
-    return HX_ERR_QUERY;
-  }
-  if (n == 0) {   // RestrictedVectorCandidates::Empty => Ok(vec![]) before any I/O
-    for (size_t b = 0; b < B; ++b) out_counts[b] = 0;
-    return HX_OK;
-  }
-  if (std::min<uint64_t>(k, n) > 800) {
-    hx_set_error("restricted vector search result count must be at most 800, got %llu",
-                 (unsigned long long)std::min<uint64_t>(k, n));
-    return HX_ERR_QUERY;
-  }
-  if (!is_set)
-    for (uint64_t i = 1; i < n; ++i)
-      if (cand_ids[i] <= cand_ids[i - 1]) {
-        hx_set_error("candidate ids must be ascending and unique (RoaringTreemap iteration order); position %llu",
-                     (unsigned long long)i);
-        return HX_ERR_INVALID_PARAMETER;
-      }
-  if (is_set && (set->ix != ix || set->generation != ix->vector_generation)) {
-    hx_set_error("candidate set does not belong to this index image (vectors were reloaded or deleted?)");
-    return HX_ERR_INVARIANT_VIOLATION;
-  }
-  HX_CUDA(cudaSetDevice(ix->device));
-  if (ix->n == 0 || !ix->populated) return answer_empty_index(ix, queries, B, out_counts, nullptr);
-  HxScratch* s = nullptr;
-  if ((rc = hx_acquire_scratch(ix, &s))) return rc;
-  ScratchGuard guard{ix, s};
-  uint32_t launches = 0;
-  if ((rc = stage_queries(ix, s, queries, B, &launches))) return rc;
-  const uint32_t* slots = nullptr;
-  if (is_set) {
-    slots = set->d_slots;
-  } else {
-    if ((rc = s->d_cand_ids.reserve(n)) || (rc = s->d_cand_slots.reserve(n))) return rc;
-    HX_CUDA(cudaMemcpyAsync(s->d_cand_ids.p, cand_ids, n * sizeof(uint64_t), cudaMemcpyHostToDevice, s->stream));
-    k_map_candidates<<<(unsigned)((n + 255) / 256), 256, 0, s->stream>>>(
-        ix->d_ids, (uint32_t)ix->n, s->d_cand_ids.p, n, s->d_cand_slots.p, ix->contiguous ? 1 : 0, ix->first_id, ix->d_deleted);
-    HX_CUDA(cudaGetLastError());
-    launches++;
-    slots = s->d_cand_slots.p;
-  }
-  // a resident set (hx_candidates_make_resident) brings its present slots, tile and view word: no compaction (and no
-  // read-back of its count), no gather, no view reduction
-  HxResident* res = is_set ? set->resident.load() : nullptr;
-  const uint32_t* d_present = nullptr;
-  size_t present = 0;
-  if (res) {
-    if ((rc = hx_resident_current(ix, res))) return rc;
-    d_present = res->slots;
-    present = res->n;
-  } else if ((rc = hx_dense_compact(ix, s, slots, n, s->stream, &d_present, &present, &launches))) {
-    return rc;
-  }
-  if ((rc = s->d_out_ids.reserve(B * (size_t)k)) || (rc = s->d_out_scores.reserve(B * (size_t)k)) ||
-      (rc = s->d_out_counts.reserve(B)))
-    return rc;
-  // below the dense path's minimum the exact scan over the same slot list: hx_search_restricted's answer and launches
-  const bool dense = present >= hx_dense_min_rows(k);
-  HxDenseCert cert;
-  if (dense && res)
-    rc = hx_dense_resident_device(ix, s, s->d_queries.p, B, k, *res, s->d_out_ids.p, s->d_out_scores.p, s->d_out_counts.p,
-                                  s->stream, s->ev0, s->ev1, &launches, exact ? &cert : nullptr);
-  else if (dense)
-    rc = hx_dense_restricted_device(ix, s, s->d_queries.p, B, k, d_present, present, s->d_out_ids.p, s->d_out_scores.p,
-                                    s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches, exact ? &cert : nullptr);
-  else
-    rc = launch_scan_select(ix, s, s->d_queries.p, B, k, slots, nullptr, true, n, n, (uint64_t)B * n, s->d_out_ids.p,
-                            s->d_out_scores.p, s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches);
-  if (rc) return rc;
-  size_t flagged = 0;
-  uint32_t err_before = 0;
-  if (exact && dense &&
-      (rc = hx_dense_rescan(ix, s, s->d_queries.p, k, d_present, present, cert, s->d_out_ids.p, s->d_out_scores.p,
-                            s->d_out_counts.p, s->stream, s->ev0, s->ev1, &launches, &flagged, &err_before)))
-    return rc;
-  if ((rc = s->h_status.reserve(B)) || (rc = s->h_err.reserve(1))) return rc;
-  if (exact && dense && out_how) HX_CUDA(cudaMemcpyAsync(out_how, cert.how, B, cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(out_ids, s->d_out_ids.p, B * (size_t)k * sizeof(uint64_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(out_scores, s->d_out_scores.p, B * (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(out_counts, s->d_out_counts.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(s->h_status.p, s->d_qstatus.p, B * sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaMemcpyAsync(s->h_err.p, s->d_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s->stream));
-  HX_CUDA(cudaStreamSynchronize(s->stream));
-  s->h_err.p[0] |= err_before;
-  for (size_t b = 0; b < B; ++b)
-    if (s->h_status.p[b] != HX_ST_OK) return status_from_word(s->h_status.p[b], b, "query");
-  if ((rc = check_device_flags(s->h_err.p[0]))) return rc;
-  float ms = 0.f;
-  if (cudaEventElapsedTime(&ms, s->ev0, s->ev1) == cudaSuccess) {   // k_dense_scores, or the exact scan below the minimum
-    ix->last_kernel_ms = ms;
-    ix->last_kernel_launches = 1;
-  }
-  if (stats) {
-    const uint64_t dim = ix->cfg.dimension, ldb = (dim + 63) / 64 * 64;
-    stats->kernel_launches = launches;
-    if (dense) {
-      stats->distance_computations = (uint64_t)B * present;
-      // gather (f32 rows in, bf16 tile and row terms out; none for a resident set), then the tile read once by the
-      // contraction
-      stats->algorithmic_bytes = (res ? 0 : present * (4 * dim + 2 * ldb + 4)) + present * 2 * ldb;
-      stats->reserved = (uint64_t)(2.0 * (double)B * (double)present * (double)ldb);   // flop of the contraction
-      if (flagged) {   // the rescanned queries' full scans over the present rows
-        stats->distance_computations += flagged * present;
-        stats->vectors_loaded += flagged * present;
-        stats->algorithmic_bytes += flagged * present * (4 * dim + (ix->cfg.metric == HX_METRIC_COSINE ? 4 : 0));
-      }
-    } else {
-      stats->distance_computations = (uint64_t)B * n;
-      stats->vectors_loaded = (uint64_t)B * n;
-      stats->algorithmic_bytes = (uint64_t)B * n * (4 * dim + (ix->cfg.metric == HX_METRIC_COSINE ? 4 : 0));
-    }
-  }
-  return HX_OK;
-}
-
-extern "C" hx_status hx_search_dense_restricted(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
-                                                const uint64_t* cand_ids, size_t n_cand, uint64_t* out_ids,
-                                                float* out_scores, uint32_t* out_counts, hx_stats* stats) {
-  return dense_restricted_host(ix, queries, B, p, cand_ids, n_cand, nullptr, false, out_ids, out_scores, out_counts, stats);
-}
-
-extern "C" hx_status hx_search_dense_restricted_set(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
-                                                    const hx_candidates* set, uint64_t* out_ids, float* out_scores,
-                                                    uint32_t* out_counts, hx_stats* stats) {
-  return dense_restricted_host(ix, queries, B, p, nullptr, 0, set, true, out_ids, out_scores, out_counts, stats);
-}
-
-extern "C" hx_status hx_search_dense_restricted_exact(hx_index* ix, const float* queries, size_t B, const hx_search_params* p,
-                                                      const uint64_t* cand_ids, size_t n_cand, uint64_t* out_ids,
-                                                      float* out_scores, uint32_t* out_counts, uint8_t* out_how,
-                                                      hx_stats* stats) {
-  return dense_restricted_host(ix, queries, B, p, cand_ids, n_cand, nullptr, false, out_ids, out_scores, out_counts, stats,
-                               true, out_how);
-}
-
-extern "C" hx_status hx_search_dense_restricted_exact_set(hx_index* ix, const float* queries, size_t B,
-                                                          const hx_search_params* p, const hx_candidates* set,
-                                                          uint64_t* out_ids, float* out_scores, uint32_t* out_counts,
-                                                          uint8_t* out_how, hx_stats* stats) {
-  return dense_restricted_host(ix, queries, B, p, nullptr, 0, set, true, out_ids, out_scores, out_counts, stats, true,
-                               out_how);
-}
-
-// hx_search_dense_restricted_set on device buffers, through a resident set: everything on the caller's stream, no
-// synchronisation once the view is current.  Admission is hx_search_dense_restricted_set's, in its order, then the set
-// must be resident.  d_out_how (may be null): the certificate without the rescan (0 certified, 1 not certified), or 2
-// for every query when the present rows are below hx_dense_min_rows(k) and the exact scan answered.
-extern "C" hx_status hx_search_dense_restricted_set_device(hx_index* ix, const float* d_queries, size_t B,
-                                                           const hx_search_params* p, const hx_candidates* set,
-                                                           uint64_t* d_out_ids, float* d_out_scores, uint32_t* d_out_counts,
-                                                           uint8_t* d_out_how, void* cuda_stream) {
-  if (!ix) {
-    hx_set_error("null index handle");
-    return HX_ERR_INDEX_NOT_FOUND;
-  }
-  uint32_t k, ef;
-  hx_status rc = check_params(ix, p, &k, &ef);
-  if (rc) return rc;
-  if (B == 0) return HX_OK;
-  if (!d_queries || !d_out_ids || !d_out_scores || !d_out_counts || !set) return HX_ERR_INVALID_PARAMETER;
-  if (ix->cfg.metric == HX_METRIC_MANHATTAN) {
-    hx_set_error("the L1 metric is not a contraction: use hx_search_restricted_device");
-    return HX_ERR_UNSUPPORTED;
-  }
-  cudaStream_t stream = (cudaStream_t)cuda_stream;
-  auto answer_none = [&]() -> hx_status {   // counts 0, every query "answered by the exact scan"
-    HX_CUDA(cudaSetDevice(ix->device));
-    HX_CUDA(cudaMemsetAsync(d_out_counts, 0, B * sizeof(uint32_t), stream));
-    if (d_out_how) HX_CUDA(cudaMemsetAsync(d_out_how, 2, B, stream));
-    return HX_OK;
-  };
-  const uint64_t n = set->n;
-  if (n > 1000000ull) {
-    hx_set_error("restricted vector search accepts at most 1000000 unique candidates");
-    return HX_ERR_QUERY;
-  }
-  if (n == 0) return answer_none();
-  if (std::min<uint64_t>(k, n) > 800) {
-    hx_set_error("restricted vector search result count must be at most 800, got %llu",
-                 (unsigned long long)std::min<uint64_t>(k, n));
-    return HX_ERR_QUERY;
-  }
-  if (set->ix != ix || set->generation != ix->vector_generation) {
-    hx_set_error("candidate set does not belong to this index image (vectors were reloaded or deleted?)");
-    return HX_ERR_INVARIANT_VIOLATION;
-  }
-  HxResident* res = set->resident.load();
-  if (!res) {
-    hx_set_error("hx_search_dense_restricted_set_device needs a resident set (hx_candidates_make_resident)");
-    return HX_ERR_INVALID_PARAMETER;
-  }
-  HX_CUDA(cudaSetDevice(ix->device));
-  if (ix->n == 0 || !ix->populated || res->n == 0) return answer_none();
-  if ((rc = hx_resident_current(ix, res))) return rc;
-  HxScratch* s = nullptr;
-  if ((rc = dev_scratch(ix, stream, &s))) return rc;
-  uint32_t launches = 0;
-  if ((rc = prepare_device_queries(ix, s, d_queries, B, stream, &launches))) return rc;
-  cudaEvent_t e0, e1;
-  if ((rc = s->ring_next(&e0, &e1))) return rc;
-  if (res->n < hx_dense_min_rows(k)) {   // the exact scan over the present slots
-    if (d_out_how) HX_CUDA(cudaMemsetAsync(d_out_how, 2, B, stream));
-    return launch_scan_select(ix, s, d_queries, B, k, res->slots, nullptr, true, res->n, res->n, (uint64_t)B * res->n,
-                              d_out_ids, d_out_scores, d_out_counts, stream, e0, e1, &launches);
-  }
-  HxDenseCert cert;
-  if ((rc = hx_dense_resident_device(ix, s, d_queries, B, k, *res, d_out_ids, d_out_scores, d_out_counts, stream, e0, e1,
-                                     &launches, d_out_how ? &cert : nullptr)))
-    return rc;
-  if (d_out_how) HX_CUDA(cudaMemcpyAsync(d_out_how, cert.how, B, cudaMemcpyDeviceToDevice, stream));
-  return HX_OK;
-}
+#include "hx_dense.inl"
 
 // ------------------------------------------------------------------------------------------------
 // SimHash policy mode (search.rs:595-992, policy.rs) — the production-default SearchParams

@@ -76,14 +76,59 @@ struct PinBuf {
   }
 };
 
-// dense path state cached across calls on one scratch set: encoded tensor maps, the shape they were built for
-struct HxDenseCache {
+// Tile shape of the dense path (k_dense.cu) that its host code sizes buffers by
+#define HXD_BN 256          // corpus rows per placement tile (the unit of the row interleave and of the column quarters)
+#define HXD_BK 64           // bf16 elements per k-block = 128 bytes = one swizzle atom
+// bf16 elements per row of a dense view or query tile: dim rounded up to a whole k-block
+inline uint32_t hx_dense_ldb(uint32_t dim) { return (dim + HXD_BK - 1) / HXD_BK * HXD_BK; }
+// rows of a dense view rounded up to a whole placement tile
+inline size_t hx_dense_rows_pad(size_t n) { return (n + HXD_BN - 1) / HXD_BN * HXD_BN; }
+
+// Dense path buffers of one scratch set, kept across calls
+struct HxDenseScratch {
+  // the tensor-core pass (k_dense.cu: dense_pass); each sized with 256 bytes of slack
+  DevBuf<uint16_t> q_tile;          // [B_pad][ldb] the queries in bf16
+  DevBuf<float> q_aux;              // [B_pad] their query terms
+  DevBuf<uint64_t> bucket_keys;     // [B][n_split][HXD_PARTS][HXD_T] k_dense_scores' buckets
+  DevBuf<uint64_t> sel_ids;         // [B][k'] the nominees ...
+  DevBuf<float> sel_sc;             // ... their approximate scores
+  DevBuf<uint32_t> sel_cnt;         // ... and how many per query
+  DevBuf<uint32_t> nominee_slots;   // [B][k'] ascending corpus slots of the nominees
+  DevBuf<uint64_t> nominee_offs;    // [B + 1] b * k'
+  DevBuf<uint64_t> rerank_keys;     // [B][k'] the exact re-rank's keys
+  // q_tile's pad rows and columns, q_aux's pad entries, nominee_offs and map_q are written once per (these three
+  // buffers, B, k', ldb) and re-initialised when any of them changes
+  const void* init_q_tile = nullptr;
+  const void* init_q_aux = nullptr;
+  const void* init_offs = nullptr;
+  size_t init_B = 0;
+  uint32_t init_kprime = 0, init_ldb = 0;
   alignas(64) unsigned char map_q[128];
-  alignas(64) unsigned char map_x[128];
-  size_t B = 0;
-  uint32_t kprime = 0, ldb = 0;
+  alignas(64) unsigned char map_x[128];   // keyed on the view's (rows, padded row count)
   const void* map_x_base = nullptr;
   size_t map_x_rows = 0;
+  // a candidate view gathered per call (hx_dense_gather): the compacted present slots, the bf16 tile, its row terms
+  DevBuf<uint32_t> present, present_counts;
+  DevBuf<uint16_t> view_rows;
+  DevBuf<float> view_aux;
+  // the certificate (dense_certify): per-query flags, their compaction, the view word, how
+  DevBuf<uint32_t> flag, flagged, flag_counts, view_word;
+  DevBuf<uint8_t> how;
+  // the rescan of the flagged queries (hx_dense.inl): gathered queries, headers, status words, their answers
+  DevBuf<float> rescan_q, rescan_hdr, rescan_sc;
+  DevBuf<uint32_t> rescan_status, rescan_cnt;
+  DevBuf<uint64_t> rescan_ids;
+  PinBuf<uint32_t> h_rescan;        // the flagged count and the error word before the rescan
+  void release() {
+    q_tile.release(); q_aux.release(); bucket_keys.release(); sel_ids.release(); sel_sc.release(); sel_cnt.release();
+    nominee_slots.release(); nominee_offs.release(); rerank_keys.release();
+    init_q_tile = init_q_aux = init_offs = nullptr;
+    map_x_base = nullptr;
+    present.release(); present_counts.release(); view_rows.release(); view_aux.release();
+    flag.release(); flagged.release(); flag_counts.release(); view_word.release(); how.release();
+    rescan_q.release(); rescan_hdr.release(); rescan_sc.release(); rescan_status.release(); rescan_cnt.release();
+    rescan_ids.release(); h_rescan.release();
+  }
 };
 
 // One scratch set per in-flight host call (the handle is Send+Sync like the reference's index:
@@ -115,15 +160,8 @@ struct HxScratch {
   DevBuf<unsigned long long> d_pstats; // policy counters
   DevBuf<uint64_t> d_qsim;             // query fingerprints
   bool prof_init = false;
-  DevBuf<uint8_t> misc[16];   // dense path buffers (kept across calls)
-  HxDenseCache dense;
-  // exact dense entries: certificate flags + compaction + the view word, how, and the gathered rescan queries and results
-  DevBuf<uint32_t> x_flag, x_status, x_counts;
-  DevBuf<uint8_t> x_how;
-  DevBuf<float> x_queries, x_hdr, x_scores;
-  DevBuf<uint64_t> x_ids;
-  PinBuf<uint32_t> h_x;
-  DevBuf<uint8_t> d_block;    // small calls: results packed into one block -> one device-to-host copy
+  HxDenseScratch dense;
+  DevBuf<uint8_t> d_block;   // small calls: results packed into one block -> one device-to-host copy
   PinBuf<uint8_t> h_block;
   PinBuf<uint64_t> h_ids, h_cand_offsets;
   PinBuf<float> h_scores, h_queries, h_qhdr;
@@ -238,39 +276,49 @@ hx_status hx_launch_cta_ring(hx_index* ix, const HxCtaRingCfg& c, const HxHnswAr
                              cudaStream_t stream, int* ctas_per_sm);
 bool hx_slot_of(const hx_index* ix, uint64_t id, uint32_t* slot);
 
-// The certificate of the exact dense entries (k_dense.cu: k_dense_certify), left on the call's stream for the rescan
+// implemented in k_build.cu
+hx_status hx_build_impl(hx_index* ix, const uint16_t* levels, uint64_t seed, int sequential);
+
+// ---- the dense path: k_dense.cu (kernels, views, pass, certificate), hx_dense.inl (entry points) ----
+// The corpus a tensor-core pass runs over: `n` bf16 rows in tile placement (k_to_bf16 with tiled = 1), their row terms
+// (indexed by position), and the ascending slot table that maps row w of the view to its corpus slot.  `word`: the view's
+// k_dense_view_bound word when the view holds one (null: the certificate reduces it per call).
+struct HxDenseView {
+  const void* rows = nullptr;
+  const float* aux = nullptr;
+  const uint32_t* slots = nullptr;
+  size_t n = 0;
+  const uint32_t* word = nullptr;
+};
+
+// The certificate of the exact dense entries (k_dense_certify), left on the call's stream for the rescan
 struct HxDenseCert {
-  bool small = false;                   // the view is below hx_dense_min_rows(k): the exact scan answered every query
   const uint32_t* flagged = nullptr;    // [B] the indices of the queries the certificate could not clear, ascending
   const uint32_t* n_flagged = nullptr;  // device word: how many
   const uint8_t* how = nullptr;         // [B] 0 certified, 1 flagged
 };
 
-// implemented in k_build.cu / k_dense.cu
-hx_status hx_build_impl(hx_index* ix, const uint16_t* levels, uint64_t seed, int sequential);
-// exact = false: hx_search_dense; true: hx_search_dense_exact (out_how may be null)
-hx_status hx_dense_impl(hx_index* ix, const float* queries, size_t B, const hx_search_params* p, uint64_t* out_ids,
-                        float* out_scores, uint32_t* out_counts, hx_stats* stats, bool exact = false,
-                        uint8_t* out_how = nullptr);
-// cert != null: the certificate runs after the re-rank (or cert->small is set)
-hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
-                          uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
-                          cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out, HxDenseCert* cert = nullptr);
-// hx_api.cu: the exact scan of the flagged queries over the view's ascending slot list, results scattered into the output
-// rows.  Synchronises the stream once to read the flagged count; *err_before receives the device error word as it was
-// before the scan reset it.
-hx_status hx_dense_rescan(hx_index* ix, HxScratch* s, const float* d_q, uint32_t k, const uint32_t* slots,
-                          size_t n_view, const HxDenseCert& cert, uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt,
-                          cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches, size_t* n_flagged,
-                          uint32_t* err_before);
 // rows below which the dense paths answer with the exact scan (the tensor-core pass could not fill its nominee lists)
 size_t hx_dense_min_rows(uint32_t k);
-hx_status hx_dense_compact(hx_index* ix, HxScratch* scr, const uint32_t* d_slots, size_t n, cudaStream_t stream,
-                           const uint32_t** d_present, size_t* n_present, uint32_t* launches);
-hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k,
-                                     const uint32_t* d_present, size_t n_present, uint64_t* d_out_ids, float* d_out_sc,
-                                     uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1,
-                                     uint32_t* launches, HxDenseCert* cert = nullptr);
+// The whole-corpus view: the ascending live slots and, when `rows`, the bf16 copy of the live rows.  Built on first use
+// after every mirror write (blocking on `stream`) and published under ix->dense_mu only once complete.
+hx_status hx_dense_corpus_view(hx_index* ix, bool rows, cudaStream_t stream, HxDenseView* v);
+// A per-call view over the ascending slot list `d_slots` (n entries, HX_ABSENT for ids without a row and deleted rows): the
+// present slots compacted in order (one synchronisation reads their count) and, when there are at least
+// hx_dense_min_rows(k), their rows gathered into a bf16 tile of the scratch set (v->rows stays null otherwise).
+hx_status hx_dense_gather(hx_index* ix, HxScratch* scr, const uint32_t* d_slots, size_t n, uint32_t k, cudaStream_t stream,
+                          HxDenseView* v, uint32_t* launches);
+// The tensor-core pass over a view (v.n >= hx_dense_min_rows(k), k <= 800) and the exact re-rank, then (cert != null)
+// the certificate.  The queries' exact headers and status words must be in scr->d_qhdr / d_qstatus.  Enqueued on `stream`,
+// no synchronisation; adds the launches it issues to *launches.
+hx_status hx_dense_search(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxDenseView& v,
+                          uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0,
+                          cudaEvent_t e1, uint32_t* launches, HxDenseCert* cert = nullptr);
+// hx_search_dense over every live row on device buffers (the sharded path): everything on `stream`, no synchronisation
+// once the whole-corpus view exists
+hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
+                          uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
+                          cudaEvent_t e0, cudaEvent_t e1);
 
 // The resident tensor-core view of a device candidate set (hx_candidates_make_resident): what
 // hx_search_dense_restricted_set otherwise rebuilds on every call, built once and kept by the set.  The present list never
@@ -280,20 +328,16 @@ struct HxResident {
   std::mutex mu;                     // held by a refresh; a new epoch is published under it once the tile is complete
   std::atomic<uint64_t> epoch{0};
   cudaStream_t stream = nullptr;     // builds and refreshes run here, never on a caller's stream
-  uint32_t* slots = nullptr;         // [n] the set's present slots, ascending (hx_dense_compact)
+  uint32_t* slots = nullptr;         // [n] the set's present slots, ascending
   size_t n = 0;
   void* rows = nullptr;              // [n rounded up to 256][ldb] bf16, tile placement over candidate rank (k_to_bf16)
   float* aux = nullptr;              // row terms by position, then (at the end) k_dense_view_bound's word
   uint32_t* word = nullptr;
   uint64_t bytes = 0;                // device memory held
+  HxDenseView view() const { return HxDenseView{rows, aux, slots, n, word}; }
 };
 // hx_candidates_make_resident: compaction of the set's slot list, gather, view word; blocking.  *out is set on success.
 hx_status hx_resident_build(hx_index* ix, const uint32_t* d_slots, size_t n_slots, HxResident** out);
 // the first call after a row write re-gathers the tile and the view word in place (same present list); otherwise nothing
 hx_status hx_resident_current(hx_index* ix, HxResident* r);
 void hx_resident_free(HxResident* r);
-// hx_dense_restricted_device over a resident view (r.n >= hx_dense_min_rows(k)): no compaction, no gather, and the
-// certificate reads the view word the view holds
-hx_status hx_dense_resident_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxResident& r,
-                                   uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
-                                   cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches, HxDenseCert* cert = nullptr);

@@ -222,7 +222,7 @@ static hx_status sharded_device_locked(hx_shard_group* g, int32_t path, const fl
   uint32_t* s_cnt = reinterpret_cast<uint32_t*>(g->send.p + bl.off_cnt);
   HX_CUDA(cudaEventRecord(g->ev0, stream));
   if (path == HX_SHARD_DENSE) {
-    if ((rc = hx_dense_device(g->ix, &g->scr, d_queries, B, local, s_ids, s_sc, s_cnt, stream, g->evk0, g->evk1, nullptr)))
+    if ((rc = hx_dense_device(g->ix, &g->scr, d_queries, B, local, s_ids, s_sc, s_cnt, stream, g->evk0, g->evk1)))
       return rc;
     g->kernel_timed = true;
   } else if (path == HX_SHARD_HNSW) {

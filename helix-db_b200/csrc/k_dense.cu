@@ -35,10 +35,8 @@
 #include "k_util.cuh"
 
 #define HXD_BM 128          // queries per CTA tile: two consumer warpgroups x 64 (wgmma M)
-#define HXD_BN 256          // corpus rows per placement tile (the unit of the row interleave and of the column quarters)
 #define HXD_BH 128          // corpus rows per MMA tile (wgmma N): a placement tile is contracted in two halves
-#define HXD_BK 64           // bf16 elements per k-block = 128 bytes = one swizzle atom
-#define HXD_STAGES 4
+#define HXD_STAGES 4        // (HXD_BN, HXD_BK: hx_index.hpp)
 #define HXD_PARTS 4         // 64-column quarters of a placement tile: one bucket of the fused top-T per (query, run, quarter)
 #ifndef HXD_T
 #define HXD_T 8             // best rows kept per (query, run of n-tiles, column quarter): 32 per (query, run)
@@ -601,11 +599,11 @@ static hx_status make_map(CUtensorMap* map, void* base, uint64_t rows, uint32_t 
 }
 
 // Lazily build the dense path's view of the corpus (dropped by every mirror write, hx_mirror.inl: invalidate_bf16): the
-// ascending live slots and, when `need_bf16`, the bf16 copy of the live rows compacted in slot order (deleted rows take
-// no tile column and no bucket space).  The work is enqueued on the calling stream and the pointers are published under
+// ascending live slots and, when `rows`, the bf16 copy of the live rows compacted in slot order (deleted rows take no
+// tile column and no bucket space).  The work is enqueued on the calling stream and the pointers are published under
 // ix->dense_mu only after that stream has completed it, so a caller on any other stream never reads a half-built copy,
 // and concurrent first callers build it once.
-static hx_status ensure_dense_state(hx_index* ix, uint32_t ldb, bool need_bf16, cudaStream_t stream) {
+hx_status hx_dense_corpus_view(hx_index* ix, bool rows, cudaStream_t stream, HxDenseView* v) {
   std::lock_guard<std::mutex> lk(ix->dense_mu);
   if (!ix->d_live_slots) {
     std::vector<uint32_t> live;
@@ -624,28 +622,31 @@ static hx_status ensure_dense_state(hx_index* ix, uint32_t ldb, bool need_bf16, 
     ix->d_live_slots = d;
     ix->n_live = live.size();
   }
-  if (!need_bf16 || ix->d_vec_bf16) return HX_OK;
-  const size_t n = ix->n_live, n_pad = (n + HXD_BN - 1) / HXD_BN * HXD_BN;
-  void* vb = nullptr;
-  float* aux = nullptr;
-  cudaError_t e = cudaMalloc(&vb, n_pad * (size_t)ldb * 2);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&aux, n_pad * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemsetAsync(vb, 0, n_pad * (size_t)ldb * 2, stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(aux, 0, n_pad * sizeof(float), stream);
-  if (e == cudaSuccess) {
-    k_to_bf16<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(ix->d_vec, n, ix->cfg.dimension, ix->ld, (__nv_bfloat16*)vb, ldb, aux,
-                                                          ix->cfg.metric, 1, ix->d_live_slots);
-    e = cudaGetLastError();
+  if (rows && !ix->d_vec_bf16) {
+    const uint32_t ldb = hx_dense_ldb(ix->cfg.dimension);
+    const size_t n = ix->n_live, n_pad = hx_dense_rows_pad(n);
+    void* vb = nullptr;
+    float* aux = nullptr;
+    cudaError_t e = cudaMalloc(&vb, n_pad * (size_t)ldb * 2);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&aux, n_pad * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemsetAsync(vb, 0, n_pad * (size_t)ldb * 2, stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(aux, 0, n_pad * sizeof(float), stream);
+    if (e == cudaSuccess) {
+      k_to_bf16<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(ix->d_vec, n, ix->cfg.dimension, ix->ld, (__nv_bfloat16*)vb, ldb,
+                                                            aux, ix->cfg.metric, 1, ix->d_live_slots);
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) {
+      if (vb) cudaFree(vb);
+      if (aux) cudaFree(aux);
+      hx_set_error("dense path bf16 copy: %s", cudaGetErrorString(e));
+      return e == cudaErrorMemoryAllocation ? HX_ERR_OUT_OF_MEMORY : HX_ERR_CUDA;
+    }
+    ix->d_vec_bf16 = vb;
+    ix->d_sqnorm = aux;
   }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-  if (e != cudaSuccess) {
-    if (vb) cudaFree(vb);
-    if (aux) cudaFree(aux);
-    hx_set_error("dense path bf16 copy: %s", cudaGetErrorString(e));
-    return e == cudaErrorMemoryAllocation ? HX_ERR_OUT_OF_MEMORY : HX_ERR_CUDA;
-  }
-  ix->d_vec_bf16 = vb;
-  ix->d_sqnorm = aux;
+  *v = HxDenseView{rows ? ix->d_vec_bf16 : nullptr, rows ? ix->d_sqnorm : nullptr, ix->d_live_slots, ix->n_live, nullptr};
   return HX_OK;
 }
 
@@ -655,114 +656,12 @@ static __global__ void k_dense_offsets(uint64_t* __restrict__ offs, size_t B, ui
   if (b <= B) offs[b] = b * (uint64_t)kprime;
 }
 
-static hx_status dense_check(hx_index* ix, const hx_search_params* p) {
-  if (!p || p->k == 0) {
-    hx_set_error("result count must be non-zero");
-    return HX_ERR_INVALID_PARAMETER;
-  }
-  if (p->k > 800) {
-    hx_set_error("dense search result count must be at most 800");
-    return HX_ERR_QUERY;
-  }
-  if (ix->cfg.storage != 1) {
-    hx_set_error("hx_search_dense needs hx_index_config.storage == 1 (bf16 copy of the corpus)");
-    return HX_ERR_INVALID_PARAMETER;
-  }
-  if (ix->cfg.metric == HX_METRIC_MANHATTAN) {
-    hx_set_error("the L1 metric is not a contraction: use hx_search_restricted");
-    return HX_ERR_UNSUPPORTED;
-  }
-  if (p->query_dimension != 0 && p->query_dimension != ix->cfg.dimension) {
-    hx_set_error("invalid dimension: expected %u, got %u", ix->cfg.dimension, p->query_dimension);
-    return HX_ERR_INVALID_DIMENSION;
-  }
-  return HX_OK;
-}
-
-// validation + exact headers (same order of checks as every other entry point)
-static void dense_validate(hx_index* ix, const float* d_q, size_t B, float* d_qhdr, uint32_t* d_status, cudaStream_t stream) {
-  const uint32_t dim = ix->cfg.dimension;
-  float limit = 0.f;
-  bool has_limit = false;
-  if (ix->cfg.metric == HX_METRIC_EUCLIDEAN) {
-    const double exact = std::sqrt((double)FLT_MAX / ((double)dim * 8.0));
-    limit = (float)exact;
-    if ((double)limit > exact) limit = std::nextafter(limit, 0.0f);
-    has_limit = true;
-  }
-  k_validate_and_header<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(d_q, B, dim, dim, ix->cfg.metric, limit, has_limit ? 1 : 0,
-                                                                    d_qhdr, d_status);
-}
-
-// Small corpora (see hx_dense_device): every query scans every live row with the exact kernel, keyed by position in the
-// ascending live-slot table, and keeps the k smallest (score, id) — the answer of restricted_exact_scan over all ids.
-static hx_status dense_exact_scan(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
-                                  uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
-                                  cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out) {
-  const size_t n = ix->n_live;
-  if (n == 0) {
-    HX_CUDA(cudaMemsetAsync(d_out_cnt, 0, B * sizeof(uint32_t), stream));
-    if (launches_out) *launches_out = 0;
-    return HX_OK;
-  }
-  hx_status rc;
-  DevBuf<uint8_t>& kb = scr->misc[15];   // not one of the tensor-core pass's buffers: its cached tensor maps stay valid
-  if ((rc = kb.reserve(B * n * 8)) || (rc = scr->d_qhdr.reserve(B)) || (rc = scr->d_qstatus.reserve(B)) ||
-      (rc = scr->d_err.reserve(4)))
-    return rc;
-  uint64_t* d_keys = reinterpret_cast<uint64_t*>(kb.p);
-  HX_CUDA(cudaMemsetAsync(scr->d_err.p, 0, 4, stream));
-  dense_validate(ix, d_q, B, scr->d_qhdr.p, scr->d_qstatus.p, stream);
-  HxDev dev = ix->dev();
-  HxScanArgs sa{};
-  sa.queries = d_q;
-  sa.q_hdr = scr->d_qhdr.p;
-  sa.q_status = scr->d_qstatus.p;
-  sa.B = (uint32_t)B;
-  sa.cand_slots = ix->d_live_slots;
-  sa.keys = d_keys;
-  sa.shared_set = 1;
-  sa.n_shared = n;
-  sa.chunk = 1024;
-  sa.err_flags = scr->d_err.p;
-  dim3 g((unsigned)((n + sa.chunk - 1) / sa.chunk), (unsigned)std::min<size_t>(B, 65535));
-  const uint32_t sm = ix->ld * 4u;
-  if (e0) HX_CUDA(cudaEventRecord(e0, stream));
-  if (ix->cfg.metric == HX_METRIC_COSINE) k_scan<HXM_COSINE><<<g, HX_SCAN_THREADS, sm, stream>>>(dev, sa);
-  else k_scan<HXM_EUCLIDEAN><<<g, HX_SCAN_THREADS, sm, stream>>>(dev, sa);
-  if (e1) HX_CUDA(cudaEventRecord(e1, stream));
-  HxSelectArgs s2{};
-  s2.keys = d_keys;
-  s2.cand_slots = ix->d_live_slots;
-  s2.q_status = scr->d_qstatus.p;
-  s2.B = (uint32_t)B;
-  s2.k = p->k;
-  s2.shared_set = 1;
-  s2.n_shared = n;
-  s2.out_ids = d_out_ids;
-  s2.out_scores = d_out_sc;
-  s2.out_counts = d_out_cnt;
-  k_select<<<(unsigned)std::min<size_t>(B, 65535), HX_SEL_THREADS, 0, stream>>>(dev, s2);
-  HX_CUDA(cudaGetLastError());
-  if (launches_out) *launches_out = 3;
-  return HX_OK;
-}
-
 // Small corpora get the exact scan.  The tensor-core pass hands each query at most HXD_PARTS * HXD_T = 32 nominees per run
 // of tiles, and a run is at least one 256-row tile, so a corpus of few tiles cannot fill k' = min(max(4k, 64), 800, rows)
 // nominees, and its count could fall short of min(k, rows).  From 8 * min(max(4k, 64), 800) rows on, every run but the
 // last holds a full tile (32 nominees), which covers k' (n_split below is at least k'/4 runs or every tile).  Below that
 // the exact scan costs at most 6400 rows per query.
 size_t hx_dense_min_rows(uint32_t k) { return 8 * (size_t)std::min<uint32_t>(std::max<uint32_t>(4 * k, 64), 800); }
-
-// The corpus a tensor-core pass runs over: `n` bf16 rows in tile placement (k_to_bf16 with tiled = 1), their row terms
-// (indexed by position), and the ascending slot table that maps row w of the view to its corpus slot.
-struct HxDenseView {
-  const void* rows;
-  const float* aux;
-  const uint32_t* slots;
-  size_t n;
-};
 
 // What a tensor-core pass leaves behind that bounds what it may have dropped (read by the certificate, k_dense_certify)
 struct HxDensePassOut {
@@ -774,17 +673,16 @@ struct HxDensePassOut {
   const float* q_aux;        // [B] query terms of the pass (euclidean: |q^|^2)
 };
 
-// Tensor-core nomination over the view, then the exact re-rank with the reference arithmetic.  Needs
-// n >= hx_dense_min_rows(k) and k <= 800, and the queries' exact headers and status words in scr->d_qhdr / d_qstatus.
-// Everything is enqueued on `stream`; nothing synchronises with the host (buffers, the query tensor map and the nominee
-// offsets are cached in the scratch set across calls; the corpus map is keyed on the view's (base, rows)).
-// `pass_out` (may be null) receives the pass's internal buffers; they stay valid until the scratch set's next dense pass.
+// Tensor-core nomination over the view, then the exact re-rank with the reference arithmetic (see hx_dense_search).
+// Buffers, the query tensor map and the nominee offsets are cached in scr->dense across calls; the corpus map is keyed on
+// the view's (base, rows).  `pass_out` (may be null) receives the pass's internal buffers; they stay valid until the
+// scratch set's next dense pass.
 static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxDenseView& v,
                             uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0,
-                            cudaEvent_t e1, uint32_t* launches_out, HxDensePassOut* pass_out = nullptr) {
+                            cudaEvent_t e1, uint32_t* launches, HxDensePassOut* pass_out) {
   hx_status rc;
   const uint32_t dim = ix->cfg.dimension;
-  const uint32_t ldb = (dim + HXD_BK - 1) / HXD_BK * HXD_BK;
+  const uint32_t ldb = hx_dense_ldb(dim);
   const size_t n = v.n;
   const uint32_t kcap = std::min<uint32_t>(std::max<uint32_t>(4 * k, 64), 800);
   const uint32_t m_tiles = (uint32_t)((B + HXD_BM - 1) / HXD_BM), n_tiles = (uint32_t)((n + HXD_BN - 1) / HXD_BN);
@@ -801,51 +699,37 @@ static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size
     for (uint32_t cand = n_split; cand <= std::min<uint32_t>(n_tiles, 2 * n_split); ++cand)
       if (((size_t)m_tiles * cand) % n_ctas == 0) { n_split = cand; break; }
   const size_t nkeys = B * (size_t)n_split * HXD_PARTS * HXD_T;
-  int mi = 0;
-  bool grew = false;
-  auto take = [&](size_t bytes, void** out) -> hx_status {
-    const unsigned char* before = scr->misc[mi].p;
-    hx_status r = scr->misc[mi].reserve(bytes + 256);
-    if (scr->misc[mi].p != before) grew = true;
-    *out = scr->misc[mi].p;
-    ++mi;
-    return r;
-  };
-  float *d_qaux, *d_sel_sc;
-  __nv_bfloat16* d_qb;
-  uint64_t *d_keys, *d_sel_ids, *d_keys2, *d_coffs;
-  uint32_t *d_sel_cnt, *d_cslots;
-  if ((rc = take(B_pad * (size_t)ldb * 2, (void**)&d_qb)) || (rc = take(B_pad * 4, (void**)&d_qaux)) ||
-      (rc = take(nkeys * 8, (void**)&d_keys)) || (rc = take(B * (size_t)kprime * 8, (void**)&d_sel_ids)) ||
-      (rc = take(B * (size_t)kprime * 4, (void**)&d_sel_sc)) || (rc = take(B * 4, (void**)&d_sel_cnt)) ||
-      (rc = take(B * (size_t)kprime * 4, (void**)&d_cslots)) || (rc = take((B + 1) * 8, (void**)&d_coffs)) ||
-      (rc = take(B * (size_t)kprime * 8, (void**)&d_keys2)))
+  HxDenseScratch& ds = scr->dense;
+  auto take = [](auto& buf, size_t count) { return buf.reserve(count + 256 / sizeof(*buf.p)); };   // 256 bytes of slack
+  if ((rc = take(ds.q_tile, B_pad * (size_t)ldb)) || (rc = take(ds.q_aux, B_pad)) || (rc = take(ds.bucket_keys, nkeys)) ||
+      (rc = take(ds.sel_ids, B * (size_t)kprime)) || (rc = take(ds.sel_sc, B * (size_t)kprime)) ||
+      (rc = take(ds.sel_cnt, B)) || (rc = take(ds.nominee_slots, B * (size_t)kprime)) ||
+      (rc = take(ds.nominee_offs, B + 1)) || (rc = take(ds.rerank_keys, B * (size_t)kprime)) || (rc = scr->d_err.reserve(1)))
     return rc;
-  if ((rc = scr->d_qhdr.reserve(B)) || (rc = scr->d_qstatus.reserve(B)) || (rc = scr->d_err.reserve(4))) return rc;
-  float* d_qhdr = scr->d_qhdr.p;
-  uint32_t* d_status = scr->d_qstatus.p;
+  __nv_bfloat16* d_qb = reinterpret_cast<__nv_bfloat16*>(ds.q_tile.p);
   uint32_t* d_err = scr->d_err.p;
-  HxDenseCache& dc = scr->dense;
-  const bool shape_changed = grew || dc.B != B || dc.kprime != kprime || dc.ldb != ldb;
   HX_CUDA(cudaMemsetAsync(d_err, 0, 4, stream));
-  HX_CUDA(cudaMemsetAsync(d_sel_ids, 0xFF, B * (size_t)kprime * 8, stream));   // unfilled nominee slots read as HX_ABSENT
-  if (shape_changed) {   // pad rows / pad columns of the bf16 query tile and the nominee offsets: once per shape
+  HX_CUDA(cudaMemsetAsync(ds.sel_ids.p, 0xFF, B * (size_t)kprime * 8, stream));   // unfilled nominee slots read as HX_ABSENT
+  if (ds.init_q_tile != ds.q_tile.p || ds.init_q_aux != ds.q_aux.p || ds.init_offs != ds.nominee_offs.p || ds.init_B != B ||
+      ds.init_kprime != kprime || ds.init_ldb != ldb) {
     HX_CUDA(cudaMemsetAsync(d_qb, 0, B_pad * (size_t)ldb * 2, stream));
-    HX_CUDA(cudaMemsetAsync(d_qaux, 0, B_pad * 4, stream));
-    k_dense_offsets<<<(unsigned)((B + 256) / 256), 256, 0, stream>>>(d_coffs, B, kprime);
-    if ((rc = make_map(reinterpret_cast<CUtensorMap*>(dc.map_q), d_qb, B_pad, ldb, HXD_BM))) return rc;
-    dc.B = B;
-    dc.kprime = kprime;
-    dc.ldb = ldb;
+    HX_CUDA(cudaMemsetAsync(ds.q_aux.p, 0, B_pad * 4, stream));
+    k_dense_offsets<<<(unsigned)((B + 256) / 256), 256, 0, stream>>>(ds.nominee_offs.p, B, kprime);
+    if ((rc = make_map(reinterpret_cast<CUtensorMap*>(ds.map_q), d_qb, B_pad, ldb, HXD_BM))) return rc;
+    ds.init_q_tile = ds.q_tile.p;
+    ds.init_q_aux = ds.q_aux.p;
+    ds.init_offs = ds.nominee_offs.p;
+    ds.init_B = B;
+    ds.init_kprime = kprime;
+    ds.init_ldb = ldb;
   }
-  if (dc.map_x_base != v.rows || dc.map_x_rows != n_pad) {
-    if ((rc = make_map(reinterpret_cast<CUtensorMap*>(dc.map_x), const_cast<void*>(v.rows), n_pad, ldb, HXD_BH))) return rc;   // one MMA tile = half a placement tile
-    dc.map_x_base = v.rows;
-    dc.map_x_rows = n_pad;
+  if (ds.map_x_base != v.rows || ds.map_x_rows != n_pad) {
+    if ((rc = make_map(reinterpret_cast<CUtensorMap*>(ds.map_x), const_cast<void*>(v.rows), n_pad, ldb, HXD_BH))) return rc;   // one MMA tile = half a placement tile
+    ds.map_x_base = v.rows;
+    ds.map_x_rows = n_pad;
   }
-  uint32_t launches = 0;
-  k_to_bf16<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(d_q, B, dim, dim, d_qb, ldb, d_qaux, ix->cfg.metric, 0, nullptr);
-  launches += 1;
+  k_to_bf16<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(d_q, B, dim, dim, d_qb, ldb, ds.q_aux.p, ix->cfg.metric, 0, nullptr);
+  *launches += 1;
   HX_CUDA(cudaGetLastError());
   // ---- tensor-core pass ----
   HxDenseArgs a{};
@@ -856,8 +740,8 @@ static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size
   a.n_tiles = n_tiles;
   a.n_split = n_split;
   a.row_aux = v.aux;
-  a.q_aux = d_qaux;
-  a.keys = d_keys;
+  a.q_aux = ds.q_aux.p;
+  a.keys = ds.bucket_keys.p;
   a.metric = ix->cfg.metric;
   const size_t smem = (size_t)HXD_STAGES * HXD_STAGE_BYTES + (size_t)HXD_BM * HXD_ACC_LD * 4 + HXD_BH * 4 + 2 * HXD_STAGES * 8 + 1024;
   static std::atomic<int> attr_set[64];
@@ -867,37 +751,37 @@ static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size
   }
   const uint32_t grid = (uint32_t)std::min<size_t>((size_t)m_tiles * n_split, n_ctas);
   if (e0) HX_CUDA(cudaEventRecord(e0, stream));
-  k_dense_scores<<<grid, HXD_THREADS, smem, stream>>>(*reinterpret_cast<CUtensorMap*>(dc.map_q),
-                                                      *reinterpret_cast<CUtensorMap*>(dc.map_x), a);
+  k_dense_scores<<<grid, HXD_THREADS, smem, stream>>>(*reinterpret_cast<CUtensorMap*>(ds.map_q),
+                                                      *reinterpret_cast<CUtensorMap*>(ds.map_x), a);
   if (e1) HX_CUDA(cudaEventRecord(e1, stream));
-  launches++;
+  *launches += 1;
   HX_CUDA(cudaGetLastError());
   // ---- k' nominees per query by approximate key, then the exact re-rank with the reference arithmetic ----
   HxDev dev = ix->dev();
   HxSelectArgs s1{};
-  s1.keys = d_keys;
-  s1.q_status = d_status;
+  s1.keys = ds.bucket_keys.p;
+  s1.q_status = scr->d_qstatus.p;
   s1.B = (uint32_t)B;
   s1.k = kprime;
   s1.shared_set = 2;   // keys carry rows of the bf16 copy in their low word (no candidate indirection)
   s1.n_shared = (uint64_t)n_split * HXD_PARTS * HXD_T;
-  s1.out_ids = d_sel_ids;
-  s1.out_scores = d_sel_sc;
-  s1.out_counts = d_sel_cnt;
+  s1.out_ids = ds.sel_ids.p;
+  s1.out_scores = ds.sel_sc.p;
+  s1.out_counts = ds.sel_cnt.p;
   k_select<<<(unsigned)std::min<size_t>(B, 65535), HX_SEL_THREADS, 0, stream>>>(dev, s1);
   uint32_t width = 32;
   while (width < kprime) width <<= 1;
-  k_nominee_slots<<<(unsigned)std::min<size_t>(B, 65535), HXD_SORT_THREADS, 0, stream>>>(d_sel_ids, B, kprime, width,
-                                                                                       v.slots, d_cslots);
-  launches += 2;
+  k_nominee_slots<<<(unsigned)std::min<size_t>(B, 65535), HXD_SORT_THREADS, 0, stream>>>(ds.sel_ids.p, B, kprime, width,
+                                                                                       v.slots, ds.nominee_slots.p);
+  *launches += 2;
   HxScanArgs sa{};
   sa.queries = d_q;
-  sa.q_hdr = d_qhdr;
-  sa.q_status = d_status;
+  sa.q_hdr = scr->d_qhdr.p;
+  sa.q_status = scr->d_qstatus.p;
   sa.B = (uint32_t)B;
-  sa.cand_slots = d_cslots;
-  sa.cand_offsets = d_coffs;
-  sa.keys = d_keys2;
+  sa.cand_slots = ds.nominee_slots.p;
+  sa.cand_offsets = ds.nominee_offs.p;
+  sa.keys = ds.rerank_keys.p;
   sa.shared_set = 0;
   sa.n_shared = 0;
   sa.chunk = 32 * ((kprime + 31) / 32);
@@ -909,10 +793,10 @@ static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size
     else k_scan<HXM_EUCLIDEAN><<<g, HX_SCAN_THREADS, sm, stream>>>(dev, sa);
   }
   HxSelectArgs s2{};
-  s2.keys = d_keys2;
-  s2.cand_slots = d_cslots;
-  s2.cand_offsets = d_coffs;
-  s2.q_status = d_status;
+  s2.keys = ds.rerank_keys.p;
+  s2.cand_slots = ds.nominee_slots.p;
+  s2.cand_offsets = ds.nominee_offs.p;
+  s2.q_status = scr->d_qstatus.p;
   s2.B = (uint32_t)B;
   s2.k = k;
   s2.shared_set = 0;
@@ -921,17 +805,16 @@ static hx_status dense_pass(hx_index* ix, HxScratch* scr, const float* d_q, size
   s2.out_scores = d_out_sc;
   s2.out_counts = d_out_cnt;
   k_select<<<(unsigned)std::min<size_t>(B, 65535), HX_SEL_THREADS, 0, stream>>>(dev, s2);
-  launches += 2;
+  *launches += 2;
   HX_CUDA(cudaGetLastError());
-  if (launches_out) *launches_out = launches;
-  if (pass_out) *pass_out = HxDensePassOut{d_keys, n_split, d_sel_sc, d_sel_cnt, kprime, d_qaux};
+  if (pass_out) *pass_out = HxDensePassOut{ds.bucket_keys.p, n_split, ds.sel_sc.p, ds.sel_cnt.p, kprime, ds.q_aux.p};
   return HX_OK;
 }
 
 // k_dense_view_bound over view `v` into *word (zeroed first), enqueued on `stream`
 static hx_status dense_view_word(hx_index* ix, const HxDenseView& v, uint32_t* word, cudaStream_t stream) {
   HX_CUDA(cudaMemsetAsync(word, 0, 4, stream));
-  const size_t n_pad = (v.n + HXD_BN - 1) / HXD_BN * HXD_BN;
+  const size_t n_pad = hx_dense_rows_pad(v.n);
   const unsigned grid = (unsigned)std::min<size_t>((n_pad + 255) / 256, 4 * (size_t)std::max(1, ix->sm_count));
   k_dense_view_bound<<<grid, 256, 0, stream>>>(v.aux, ix->d_hdr, v.slots, v.n, ix->cfg.metric, word);
   HX_CUDA(cudaGetLastError());
@@ -939,22 +822,21 @@ static hx_status dense_view_word(hx_index* ix, const HxDenseView& v, uint32_t* w
 }
 
 // The certificate after a pass over view `v` (see k_dense_certify), then the order-preserving compaction of the flagged
-// query indices.  Enqueued on `stream`, no synchronisation.  Buffers: the scratch set's x_flag / x_how, none of the pass's.
-// `resident_word`: the view's word as a resident view holds it (null: reduced here, one more launch).
+// query indices.  Enqueued on `stream`, no synchronisation.  The view's word is reduced here (one more launch) unless the
+// view holds it.
 static hx_status dense_certify(hx_index* ix, HxScratch* scr, size_t B, uint32_t k, const HxDenseView& v,
                                const HxDensePassOut& po, const float* d_out_sc, const uint32_t* d_out_cnt, HxDenseCert* cert,
-                               cudaStream_t stream, uint32_t* launches, const uint32_t* resident_word = nullptr) {
+                               cudaStream_t stream, uint32_t* launches) {
   hx_status rc;
+  HxDenseScratch& ds = scr->dense;
   const size_t tiles = (B + HXD_CPT_TILE - 1) / HXD_CPT_TILE;
-  if ((rc = scr->x_flag.reserve(2 * B + tiles + 2)) || (rc = scr->x_how.reserve(B))) return rc;
-  uint32_t* flag = scr->x_flag.p;          // [B] per query
-  uint32_t* flagged = flag + B;            // [B] compacted
-  uint32_t* counts = flagged + B;          // [tiles] + the total
-  const uint32_t* view_word = resident_word;
+  if ((rc = ds.flag.reserve(B)) || (rc = ds.flagged.reserve(B)) || (rc = ds.flag_counts.reserve(tiles + 1)) ||
+      (rc = ds.how.reserve(B)))
+    return rc;
+  const uint32_t* view_word = v.word;
   if (!view_word) {
-    uint32_t* w = counts + tiles + 1;
-    if ((rc = dense_view_word(ix, v, w, stream))) return rc;
-    view_word = w;
+    if ((rc = ds.view_word.reserve(1)) || (rc = dense_view_word(ix, v, ds.view_word.p, stream))) return rc;
+    view_word = ds.view_word.p;
     ++*launches;
   }
   HxCertArgs a{};
@@ -972,132 +854,87 @@ static hx_status dense_certify(hx_index* ix, HxScratch* scr, size_t B, uint32_t 
   a.B = (uint32_t)B;
   a.k = k;
   a.dim = ix->cfg.dimension;
-  a.ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
+  a.ldb = hx_dense_ldb(ix->cfg.dimension);
   a.metric = ix->cfg.metric;
-  a.flag = flag;
-  a.how = scr->x_how.p;
+  a.flag = ds.flag.p;
+  a.how = ds.how.p;
+  uint32_t* counts = ds.flag_counts.p;   // [tiles] per-tile counts, then the total
   k_dense_certify<<<(unsigned)((B + 7) / 8), 256, 0, stream>>>(a);
-  k_compact_count<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(flag, B, counts);
-  k_compact_scatter<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(flag, B, counts, flagged, counts + tiles);
+  k_compact_count<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(ds.flag.p, B, counts);
+  k_compact_scatter<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(ds.flag.p, B, counts, ds.flagged.p, counts + tiles);
   HX_CUDA(cudaGetLastError());
   *launches += 3;
-  cert->small = false;
-  cert->flagged = flagged;
+  cert->flagged = ds.flagged.p;
   cert->n_flagged = counts + tiles;
-  cert->how = scr->x_how.p;
+  cert->how = ds.how.p;
   return HX_OK;
 }
 
-// hx_search_dense over every live row.  Everything below is enqueued on `stream`; nothing synchronises with the host once
-// the dense state exists.  d_queries: B x dim f32 on the device.  Per-query validation status is left in s->d_qstatus
-// (a query that fails validation yields count 0); error flags accumulate in s->d_err[0].
-hx_status hx_dense_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, const hx_search_params* p,
-                          uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
-                          cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches_out, HxDenseCert* cert) {
-  hx_status rc = dense_check(ix, p);
-  if (rc) return rc;
-  if (B == 0) return HX_OK;
-  if (ix->n == 0 || !ix->populated) {
-    HX_CUDA(cudaMemsetAsync(d_out_cnt, 0, B * sizeof(uint32_t), stream));
-    return HX_OK;
-  }
-  const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
-  if ((rc = ensure_dense_state(ix, ldb, false, stream))) return rc;
-  const size_t n = ix->n_live;   // rows of the bf16 copy: the live rows, compacted
-  if (n < hx_dense_min_rows(p->k)) {
-    if (cert) cert->small = true;
-    return dense_exact_scan(ix, scr, d_q, B, p, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out);
-  }
-  if ((rc = ensure_dense_state(ix, ldb, true, stream))) return rc;
-  if ((rc = scr->d_qhdr.reserve(B)) || (rc = scr->d_qstatus.reserve(B))) return rc;
-  dense_validate(ix, d_q, B, scr->d_qhdr.p, scr->d_qstatus.p, stream);
-  const HxDenseView v{ix->d_vec_bf16, ix->d_sqnorm, ix->d_live_slots, n};
+hx_status hx_dense_search(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxDenseView& v,
+                          uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0,
+                          cudaEvent_t e1, uint32_t* launches, HxDenseCert* cert) {
   HxDensePassOut po{};
-  rc = dense_pass(ix, scr, d_q, B, p->k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches_out, cert ? &po : nullptr);
-  if (!rc && launches_out) *launches_out += 1;
-  if (!rc && cert) {
-    uint32_t l = 0;
-    rc = dense_certify(ix, scr, B, p->k, v, po, d_out_sc, d_out_cnt, cert, stream, &l);
-    if (launches_out) *launches_out += l;
-  }
-  return rc;
+  hx_status rc = dense_pass(ix, scr, d_q, B, k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, launches,
+                            cert ? &po : nullptr);
+  if (rc || !cert) return rc;
+  return dense_certify(ix, scr, B, k, v, po, d_out_sc, d_out_cnt, cert, stream, launches);
 }
 
-// hx_search_dense_restricted, step 1: the present entries of the ascending candidate slot list `d_slots` (n entries,
-// HX_ABSENT for ids without a row and for deleted rows), compacted in order into scratch.  Synchronises the stream to read
-// the count back (4 bytes).
-hx_status hx_dense_compact(hx_index* ix, HxScratch* scr, const uint32_t* d_slots, size_t n, cudaStream_t stream,
-                           const uint32_t** d_present, size_t* n_present, uint32_t* launches) {
+// The present entries of the ascending candidate slot list `d_slots` (n entries, HX_ABSENT for ids without a row and for
+// deleted rows), compacted in order into scr->dense.present.  Synchronises the stream to read the count back (4 bytes).
+static hx_status dense_compact(HxScratch* scr, const uint32_t* d_slots, size_t n, cudaStream_t stream, size_t* n_present,
+                               uint32_t* launches) {
   hx_status rc;
+  HxDenseScratch& ds = scr->dense;
   const size_t tiles = (n + HXD_CPT_TILE - 1) / HXD_CPT_TILE;
-  if ((rc = scr->misc[11].reserve(n * 4)) || (rc = scr->misc[12].reserve((tiles + 1) * 4)) || (rc = scr->h_err.reserve(1)))
-    return rc;
-  uint32_t* out = reinterpret_cast<uint32_t*>(scr->misc[11].p);
-  uint32_t* counts = reinterpret_cast<uint32_t*>(scr->misc[12].p);   // [tiles] per-tile counts, then the total
+  if ((rc = ds.present.reserve(n)) || (rc = ds.present_counts.reserve(tiles + 1)) || (rc = scr->h_err.reserve(1))) return rc;
+  uint32_t* counts = ds.present_counts.p;   // [tiles] per-tile counts, then the total
   k_compact_count<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(d_slots, n, counts);
-  k_compact_scatter<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(d_slots, n, counts, out, counts + tiles);
+  k_compact_scatter<<<(unsigned)tiles, HXD_CPT_THREADS, 0, stream>>>(d_slots, n, counts, ds.present.p, counts + tiles);
   HX_CUDA(cudaGetLastError());
   *launches += 2;
   HX_CUDA(cudaMemcpyAsync(scr->h_err.p, counts + tiles, 4, cudaMemcpyDeviceToHost, stream));
   HX_CUDA(cudaStreamSynchronize(stream));
-  *d_present = out;
   *n_present = scr->h_err.p[0];
   return HX_OK;
 }
 
-// The tensor-core pass over a candidate view, then (cert != null) the certificate; `view_word` as dense_certify's
-// resident_word.  Adds the launches it issues to *launches.
-static hx_status dense_view_search(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxDenseView& v,
-                                   const uint32_t* view_word, uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt,
-                                   cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches,
-                                   HxDenseCert* cert) {
+// The gather converts the present rows from the f32 rows into a bf16 tile of this scratch set's own (k_to_bf16: tile
+// placement over candidate RANK, cosine power-of-two scaling, row terms); the whole-corpus bf16 copy is neither built nor
+// read.
+hx_status hx_dense_gather(hx_index* ix, HxScratch* scr, const uint32_t* d_slots, size_t n, uint32_t k, cudaStream_t stream,
+                          HxDenseView* v, uint32_t* launches) {
   hx_status rc;
-  uint32_t pass_launches = 0;
-  HxDensePassOut po{};
-  if ((rc = dense_pass(ix, scr, d_q, B, k, v, d_out_ids, d_out_sc, d_out_cnt, stream, e0, e1, &pass_launches,
-                       cert ? &po : nullptr)))
-    return rc;
-  *launches += pass_launches;
-  if (cert) return dense_certify(ix, scr, B, k, v, po, d_out_sc, d_out_cnt, cert, stream, launches, view_word);
-  return HX_OK;
-}
-
-// hx_search_dense_restricted, step 2 (n_present >= hx_dense_min_rows(k)): the present rows, converted from the f32 rows into
-// a bf16 tile of this scratch set's own (k_to_bf16: tile placement over candidate RANK, cosine power-of-two scaling, row
-// terms), then the tensor-core pass over that tile with the compacted slots as its slot table.  The whole-corpus bf16 copy
-// is neither built nor read.  The queries' headers and status words must be in scr->d_qhdr / d_qstatus.
-hx_status hx_dense_restricted_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k,
-                                     const uint32_t* d_present, size_t n_present, uint64_t* d_out_ids, float* d_out_sc,
-                                     uint32_t* d_out_cnt, cudaStream_t stream, cudaEvent_t e0, cudaEvent_t e1,
-                                     uint32_t* launches, HxDenseCert* cert) {
-  hx_status rc;
-  const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
-  const size_t n_pad = (n_present + HXD_BN - 1) / HXD_BN * HXD_BN;
-  if ((rc = scr->misc[9].reserve(n_pad * (size_t)ldb * 2)) || (rc = scr->misc[10].reserve(n_pad * 4))) return rc;
-  void* tile = scr->misc[9].p;
-  float* aux = reinterpret_cast<float*>(scr->misc[10].p);
+  HxDenseScratch& ds = scr->dense;
+  size_t present = 0;
+  if ((rc = dense_compact(scr, d_slots, n, stream, &present, launches))) return rc;
+  *v = HxDenseView{nullptr, nullptr, ds.present.p, present, nullptr};
+  if (present < hx_dense_min_rows(k)) return HX_OK;
+  const uint32_t ldb = hx_dense_ldb(ix->cfg.dimension);
+  const size_t n_pad = hx_dense_rows_pad(present);
+  if ((rc = ds.view_rows.reserve(n_pad * (size_t)ldb)) || (rc = ds.view_aux.reserve(n_pad))) return rc;
   // the positions of the last placement tile that no candidate fills read as zero rows
-  HX_CUDA(cudaMemsetAsync(static_cast<unsigned char*>(tile) + (n_pad - HXD_BN) * (size_t)ldb * 2, 0, (size_t)HXD_BN * ldb * 2,
-                          stream));
-  k_to_bf16<<<(unsigned)((n_present + 7) / 8), 256, 0, stream>>>(ix->d_vec, n_present, ix->cfg.dimension, ix->ld,
-                                                                 (__nv_bfloat16*)tile, ldb, aux, ix->cfg.metric, 1, d_present);
+  HX_CUDA(cudaMemsetAsync(ds.view_rows.p + (n_pad - HXD_BN) * (size_t)ldb, 0, (size_t)HXD_BN * ldb * 2, stream));
+  k_to_bf16<<<(unsigned)((present + 7) / 8), 256, 0, stream>>>(ix->d_vec, present, ix->cfg.dimension, ix->ld,
+                                                               (__nv_bfloat16*)ds.view_rows.p, ldb, ds.view_aux.p,
+                                                               ix->cfg.metric, 1, ds.present.p);
   HX_CUDA(cudaGetLastError());
   *launches += 1;
-  return dense_view_search(ix, scr, d_q, B, k, HxDenseView{tile, aux, d_present, n_present}, nullptr, d_out_ids, d_out_sc,
-                           d_out_cnt, stream, e0, e1, launches, cert);
+  v->rows = ds.view_rows.p;
+  v->aux = ds.view_aux.p;
+  return HX_OK;
 }
 
 // ---- resident candidate views (hx_candidates_make_resident) -------------------------------------------------------------------
 // The tile, its row terms and the view word of a resident view, from the current f32 rows of its present slots: the same
-// kernels, on the same rows, as hx_dense_restricted_device and dense_certify run per call, so a search through the view
-// returns the non-resident set's answer bit for bit.  Enqueued on r->stream, then ONE synchronisation.
+// kernels, on the same rows, as hx_dense_gather and dense_certify run per call, so a search through the view returns the
+// non-resident set's answer bit for bit.  Enqueued on r->stream, then ONE synchronisation.
 static hx_status resident_fill(hx_index* ix, HxResident* r) {
-  const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
   k_to_bf16<<<(unsigned)((r->n + 7) / 8), 256, 0, r->stream>>>(ix->d_vec, r->n, ix->cfg.dimension, ix->ld,
-                                                                (__nv_bfloat16*)r->rows, ldb, r->aux, ix->cfg.metric, 1,
-                                                                r->slots);
+                                                                (__nv_bfloat16*)r->rows, hx_dense_ldb(ix->cfg.dimension),
+                                                                r->aux, ix->cfg.metric, 1, r->slots);
   HX_CUDA(cudaGetLastError());
-  hx_status rc = dense_view_word(ix, HxDenseView{r->rows, r->aux, r->slots, r->n}, r->word, r->stream);
+  hx_status rc = dense_view_word(ix, r->view(), r->word, r->stream);
   if (rc) return rc;
   HX_CUDA(cudaStreamSynchronize(r->stream));
   return HX_OK;
@@ -1122,18 +959,17 @@ hx_status hx_resident_build(hx_index* ix, const uint32_t* d_slots, size_t n_slot
     hx_status rc = hx_acquire_scratch(ix, &s);
     if (rc) return rc;
     struct Rel { hx_index* ix; HxScratch* s; ~Rel() { hx_release_scratch(ix, s); } } rel{ix, s};
-    const uint32_t* d_present = nullptr;
     uint32_t launches = 0;
-    if ((rc = hx_dense_compact(ix, s, d_slots, n_slots, r->stream, &d_present, &r->n, &launches))) return rc;
+    if ((rc = dense_compact(s, d_slots, n_slots, r->stream, &r->n, &launches))) return rc;
     if (r->n) {
-      const uint32_t ldb = (ix->cfg.dimension + HXD_BK - 1) / HXD_BK * HXD_BK;
-      const size_t n_pad = (r->n + HXD_BN - 1) / HXD_BN * HXD_BN;
+      const uint32_t ldb = hx_dense_ldb(ix->cfg.dimension);
+      const size_t n_pad = hx_dense_rows_pad(r->n);
       HX_CUDA(cudaMalloc((void**)&r->slots, r->n * 4));
       HX_CUDA(cudaMalloc(&r->rows, n_pad * (size_t)ldb * 2));
       HX_CUDA(cudaMalloc((void**)&r->aux, (n_pad + 1) * 4));
       r->word = reinterpret_cast<uint32_t*>(r->aux + n_pad);
       r->bytes = n_pad * (uint64_t)(2 * ldb + 4) + 4 * (uint64_t)r->n + 4;
-      HX_CUDA(cudaMemcpyAsync(r->slots, d_present, r->n * 4, cudaMemcpyDeviceToDevice, r->stream));
+      HX_CUDA(cudaMemcpyAsync(r->slots, s->dense.present.p, r->n * 4, cudaMemcpyDeviceToDevice, r->stream));
       // the positions of the last placement tile that no candidate fills read as zero rows, for good: refreshes rewrite
       // the present positions only
       HX_CUDA(cudaMemsetAsync(r->rows, 0, n_pad * (size_t)ldb * 2, r->stream));
@@ -1147,9 +983,9 @@ hx_status hx_resident_build(hx_index* ix, const uint32_t* d_slots, size_t n_slot
   return HX_OK;
 }
 
-// The pattern of ensure_dense_state: a caller that finds the view stale takes the view's mutex, re-checks, re-gathers on the
-// view's own stream, synchronises once and only then publishes the epoch; concurrent first callers wait on the mutex and
-// find it current, so the tile is rebuilt once and never read half built.  In place: a stream-ordered search that still
+// The pattern of hx_dense_corpus_view: a caller that finds the view stale takes the view's mutex, re-checks, re-gathers on
+// the view's own stream, synchronises once and only then publishes the epoch; concurrent first callers wait on the mutex
+// and find it current, so the tile is rebuilt once and never read half built.  In place: a stream-ordered search that still
 // reads the tile counts as overlapping the row write that made it stale (patch calls must not overlap searches).
 hx_status hx_resident_current(hx_index* ix, HxResident* r) {
   const uint64_t want = ix->content_epoch.load(std::memory_order_acquire);
@@ -1159,89 +995,5 @@ hx_status hx_resident_current(hx_index* ix, HxResident* r) {
   hx_status rc = resident_fill(ix, r);
   if (rc) return rc;
   r->epoch.store(want, std::memory_order_release);
-  return HX_OK;
-}
-
-hx_status hx_dense_resident_device(hx_index* ix, HxScratch* scr, const float* d_q, size_t B, uint32_t k, const HxResident& r,
-                                   uint64_t* d_out_ids, float* d_out_sc, uint32_t* d_out_cnt, cudaStream_t stream,
-                                   cudaEvent_t e0, cudaEvent_t e1, uint32_t* launches, HxDenseCert* cert) {
-  return dense_view_search(ix, scr, d_q, B, k, HxDenseView{r.rows, r.aux, r.slots, r.n}, r.word, d_out_ids, d_out_sc,
-                           d_out_cnt, stream, e0, e1, launches, cert);
-}
-
-// Host-buffer entry point: a private stream + scratch set per call, the queries cross PCIe with one async copy, results
-// and per-query status come back with four, ONE stream synchronisation.  `exact` (hx_search_dense_exact): the certificate
-// follows the re-rank and the queries it cannot clear are rescanned (hx_dense_rescan: one more synchronisation, for the
-// flagged count); out_how (may be null) receives 0 / 1 per query, or 2 for every query when the exact scan answered all.
-hx_status hx_dense_impl(hx_index* ix, const float* queries, size_t B, const hx_search_params* p, uint64_t* out_ids,
-                        float* out_scores, uint32_t* out_counts, hx_stats* stats, bool exact, uint8_t* out_how) {
-  hx_status rc = dense_check(ix, p);
-  if (rc) return rc;
-  if (stats) memset(stats, 0, sizeof(*stats));
-  if (B == 0) return HX_OK;
-  if (!queries || !out_ids || !out_scores || !out_counts) return HX_ERR_INVALID_PARAMETER;
-  if (exact && out_how) memset(out_how, 2, B);
-  if (ix->n == 0 || !ix->populated) {
-    for (size_t b = 0; b < B; ++b) out_counts[b] = 0;
-    return HX_OK;
-  }
-  const uint32_t dim = ix->cfg.dimension, k = p->k;
-  HxScratch* scr = nullptr;
-  if ((rc = hx_acquire_scratch(ix, &scr))) return rc;
-  struct Rel { hx_index* ix; HxScratch* s; ~Rel() { hx_release_scratch(ix, s); } } rel{ix, scr};
-  if ((rc = scr->d_queries.reserve(B * (size_t)dim)) || (rc = scr->d_out_ids.reserve(B * (size_t)k)) ||
-      (rc = scr->d_out_scores.reserve(B * (size_t)k)) || (rc = scr->d_out_counts.reserve(B)) ||
-      (rc = scr->h_status.reserve(B)) || (rc = scr->h_err.reserve(1)))
-    return rc;
-  cudaStream_t st = scr->stream;
-  HX_CUDA(cudaMemcpyAsync(scr->d_queries.p, queries, B * (size_t)dim * 4, cudaMemcpyHostToDevice, st));
-  uint32_t launches = 0;
-  HxDenseCert cert;
-  if ((rc = hx_dense_device(ix, scr, scr->d_queries.p, B, p, scr->d_out_ids.p, scr->d_out_scores.p, scr->d_out_counts.p, st,
-                            scr->ev0, scr->ev1, &launches, exact ? &cert : nullptr)))
-    return rc;
-  size_t flagged = 0;
-  uint32_t err_before = 0;
-  if (exact && !cert.small &&
-      (rc = hx_dense_rescan(ix, scr, scr->d_queries.p, k, ix->d_live_slots, ix->n_live, cert, scr->d_out_ids.p,
-                            scr->d_out_scores.p, scr->d_out_counts.p, st, scr->ev0, scr->ev1, &launches, &flagged,
-                            &err_before)))
-    return rc;
-  HX_CUDA(cudaMemcpyAsync(out_ids, scr->d_out_ids.p, B * (size_t)k * 8, cudaMemcpyDeviceToHost, st));
-  HX_CUDA(cudaMemcpyAsync(out_scores, scr->d_out_scores.p, B * (size_t)k * 4, cudaMemcpyDeviceToHost, st));
-  HX_CUDA(cudaMemcpyAsync(out_counts, scr->d_out_counts.p, B * 4, cudaMemcpyDeviceToHost, st));
-  HX_CUDA(cudaMemcpyAsync(scr->h_status.p, scr->d_qstatus.p, B * 4, cudaMemcpyDeviceToHost, st));
-  HX_CUDA(cudaMemcpyAsync(scr->h_err.p, scr->d_err.p, 4, cudaMemcpyDeviceToHost, st));
-  if (exact && !cert.small && out_how) HX_CUDA(cudaMemcpyAsync(out_how, cert.how, B, cudaMemcpyDeviceToHost, st));
-  HX_CUDA(cudaStreamSynchronize(st));
-  scr->h_err.p[0] |= err_before;
-  for (size_t b = 0; b < B; ++b)
-    if (scr->h_status.p[b] != HX_ST_OK) {
-      const uint32_t w = scr->h_status.p[b], code = w >> 24;
-      hx_set_error_index(w & 0xffffffu);
-      hx_set_error("query %zu failed validation (code %u)", b, code);
-      return code == HX_ST_COMPONENT ? HX_ERR_INVALID_VECTOR_COMPONENT
-                                     : (code == HX_ST_ZERO_NORM ? HX_ERR_ZERO_NORM_COSINE : HX_ERR_MAGNITUDE_EXCEEDED);
-    }
-  if (scr->h_err.p[0] & HXF_INVALID_SCORE) {
-    hx_set_error("vector distance kernel emitted an invalid score");
-    return HX_ERR_INVARIANT_VIOLATION;
-  }
-  float ms = 0.f;
-  if (cudaEventElapsedTime(&ms, scr->ev0, scr->ev1) == cudaSuccess) {
-    ix->last_kernel_ms = ms;
-    ix->last_kernel_launches = 1;
-  }
-  if (stats) {
-    const uint32_t ldb = (dim + HXD_BK - 1) / HXD_BK * HXD_BK;
-    stats->kernel_launches = launches;
-    stats->distance_computations = (uint64_t)B * ix->n;
-    stats->algorithmic_bytes = (uint64_t)ix->n * ldb * 2;   // corpus streamed once; the bound is the tensor pipe: 2*B*N*d flop
-    stats->reserved = (uint64_t)(2.0 * (double)B * (double)ix->n * (double)ldb);   // flop of the contraction
-    if (flagged) {   // the rescanned queries' full scans
-      stats->distance_computations += flagged * ix->n_live;
-      stats->algorithmic_bytes += flagged * ix->n_live * (4ull * dim + (ix->cfg.metric == HX_METRIC_COSINE ? 4 : 0));
-    }
-  }
   return HX_OK;
 }
